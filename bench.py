@@ -1,25 +1,30 @@
 #!/usr/bin/env python
 """bench.py - cells x genes / s through the smooth block + HMM (BASELINE.json metric).
 
-    python bench.py [--config c2|c3|c4|c5] [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--config c2|c3|c4|c5] [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over the workload: run() steps 4, 8-12, 14 (fused smooth block) followed by
 step 17 (per-cell Viterbi) on a synthetic depth-normalised matrix; c4 adds apply_median_filtering.
 
 Configs are BASELINE.json's (SURVEY section 8d), seeds 20260922 + index:
   c2  10 000 cells x 10 000 genes, i6                      (the reference's CPU-runnable size)
-  c3  100 000 x 10 000, i6   <- DEFAULT: the configuration the metric is quoted on; fits one B200 (8 GB in, 8 GB out)
+  c3  100 000 x 10 000, i6   <- DEFAULT: the configuration the metric is quoted on; fits one H100 (8 GB in, 8 GB out)
   c4  100 000 x 10 000, i3 (mu / sigma from the reference cells) + apply_median_filtering over 50-500-cell subclusters
-  c5  500 000 x 20 000, i6, 8 x B200; with fewer ranks the same shape at 62 500 cells per rank (labelled as such)
+  c5  500 000 x 20 000, i6, 8 GPUs; with fewer ranks the same shape at 62 500 cells per rank (labelled as such)
 N > 1 (torchrun, one rank per GPU) STRONG-scales the configuration: the cells are cut into N shards, the only exchange
 is one NCCL all-gather of reference chunk sums behind each of the two reference-mean steps (c4: plus the mu / sigma
 pairs and the 4-cell halos of the reference groups for the median filter).  `--scaling weak` keeps the per-rank cells.
-Inputs are far larger than the 126 MB L2 (>= 0.8 GB per pass), so consecutive timed steps cannot hit in cache.
+Inputs are far larger than the 50 MB L2 of an H100 (>= 0.8 GB per pass), so consecutive timed steps cannot hit in cache.
 
 Prints ONE JSON line (rank 0).  `value` = device-resident throughput (CUDA events, max over ranks); `e2e` = the same
 metric through the host-pointer C ABI from PAGEABLE host memory (what an R matrix is), H2D and D2H inside the timed
-region; `roofline` = the dominant kernel against measured HBM bandwidth; `cpu_baseline` = the C oracle port on the host
-cores over a bounded sample.
+region; `roofline` = the dominant kernel against HBM bandwidth; `cpu_baseline` = the C oracle port on the host
+cores over a bounded sample; `device` = the GPU's name and power limit, which every number of the line depends on.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed for a fixed, seeded sample of rank
+0's cells (at most 64 MB in all): smoothed.npy (float64, cells x genes), states.npy (float32), median_filtered.npy (c4,
+float64) and cells.npy (the sampled global cell indices).  The inputs depend only on the arguments, so two builds of the
+project can be compared output for output.
 
 `--impl reference` times the CPU restatement of the reference's algorithm (oracle/; the reference itself is interpreted
 R: when `Rscript` and the reference's R sources are reachable the arm source()s them instead, kind "reference-R") with
@@ -79,17 +84,6 @@ def ref_groups_global(C_total: int):
     return [np.arange(0, a, dtype=np.int64), np.arange(a, b, dtype=np.int64)]
 
 
-def ncu_traffic(kernel, config, world):
-    """DRAM bytes per launch of `kernel` on `config` from the committed ncu --set full capture
-    (profiles/r02_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum of one launch), or None."""
-    if world != 1:
-        return None
-    try:
-        return float(json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))[config][kernel]["dram_bytes_per_launch"])
-    except Exception:
-        return None
-
-
 def measured_peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -97,11 +91,11 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
-    """Clock / throttle-reason sampling during the timed region (B200_PROFILING.md clocks line).
+    """Clock / throttle-reason sampling during the timed region.
 
     Two sources run side by side from before the warm-up until after the timed region: an `nvidia-smi -lms 20`
     child writing CSV to a temp file, and an NVML polling thread in this process (pynvml, same counters).  Samples
@@ -261,7 +255,7 @@ def workload_config(args, cfg, G, C_total, world, note):
             "config": args.config, "cells": C_total, "cells_per_gpu": per, "genes": G, "window_length": 101,
             "hmm": f"{cfg['hmm']} per cell, t=1e-6" + (", mu / sigma from the reference cells, i3_p_val 0.05" if cfg["hmm"] == "i3" else ""),
             "reference_cells": "first 10 % in two groups (6 % / 4 %)", "sharding": f"cells over {world} GPU(s)",
-            "l2": "inputs (%.2f GB/GPU/pass) exceed the 126 MB L2; no explicit flush" % (per * G * 8 / 1e9)}
+            "l2": "inputs (%.2f GB/GPU/pass) exceed the 50 MB L2; no explicit flush" % (per * G * 8 / 1e9)}
 
 
 def i6_model():
@@ -482,6 +476,8 @@ def main():
     ap.add_argument("--ref-sample-cells", type=int, default=512)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
@@ -596,6 +592,8 @@ def main():
             raise SystemExit("non-finite / underflow flag raised during the benchmark")
     smin, smax = int(states.min().item()), int(states.max().item())
     assert 1 <= smin and smax <= (6 if cfg["hmm"] == "i6" else 3), (smin, smax)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, cells, Y, states, Fext[:C_local] if cfg["median_filter"] else None, G)
 
     # ---- end to end through the host-facing API from PAGEABLE host memory, copies inside the timed region ----
     e2e = None
@@ -623,7 +621,7 @@ def main():
         def roof(name, kernel, nbytes, ms, note, **extra):
             ach = nbytes / (ms * 1e-3) / 1e9
             d = {"kernel": f"{kernel} ({100 * ms / ms_step:.0f} % of the step)", "bound": "hbm", "achieved": ach, "peak": peak,
-                 "unit": "GB/s", "frac": ach / peak, "traffic": ncu_traffic(name, args.config, world), "peak_source": peak_src,
+                 "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src,
                  "algorithmic_bytes_per_launch": nbytes, "ms_per_launch": ms, "note": note}
             d.update(extra)
             return d
@@ -641,7 +639,7 @@ def main():
             "steps": steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": args.scaling_label, "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": workload_config(args, cfg, G, C_total, world, note),
-            "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
+            "device": device_info(local_rank), "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
             "roofline": {"cell_pipeline pass 2": r_p2, "viterbi": r_hmm, "median_filter": r_mf}[dominant],
             "roofline_cell_pipeline": r_p2, "roofline_hmm": r_hmm,
             "roofline_smooth_block": {"kernels": "group partial sums + bounds + cell_pipeline pass 1 (reference cells) + pass 2",
@@ -658,6 +656,38 @@ def main():
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def device_info(gpu_index):
+    """Name and power limit of the GPU the line was measured on (None where nvidia-smi cannot say)."""
+    out = {"name": None, "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                           capture_output=True, text=True, timeout=30)
+        name, limit = r.stdout.strip().rsplit(",", 1)
+        out["name"] = name.strip()
+        out["power_limit_w"] = float(limit)
+    except Exception:
+        pass
+    return out
+
+
+DUMP_BYTES = 48 << 20
+
+
+def dump_outputs(d, cells, Y, states, F, G):
+    """--dump-outputs: the last step's outputs for a fixed, seeded sample of cells, at most DUMP_BYTES in all."""
+    import torch
+    per_cell = G * (8 + 4 + (8 if F is not None else 0)) + 8
+    n = max(1, min(len(cells), DUMP_BYTES // per_cell))
+    pick = np.sort(np.random.default_rng(SEED0).choice(len(cells), size=n, replace=False))
+    idx = torch.as_tensor(pick, device=Y.device)
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "cells.npy"), np.asarray(cells)[pick].astype(np.float64))
+    np.save(os.path.join(d, "smoothed.npy"), Y.index_select(0, idx).cpu().numpy().astype(np.float64))
+    np.save(os.path.join(d, "states.npy"), states.index_select(0, idx).cpu().numpy().astype(np.float32))
+    if F is not None:
+        np.save(os.path.join(d, "median_filtered.npy"), F.index_select(0, idx).cpu().numpy().astype(np.float64))
 
 
 def run_e2e(args, cfg, eng, api, X, Yext, Fext, states, cs, cl, ref_local, sub_local, plan, model6, G, C_total, C_local, world, barrier):

@@ -1,5 +1,5 @@
 /*
- * infercnv_b200.h - C ABI of libinfercnv_b200.so: the B200 (sm_100a) drop-in for the
+ * infercnv_b200.h - C ABI of libinfercnv_b200.so: the H100 (sm_90a) drop-in for the
  * smoothing + HMM hot path of broadinstitute/infercnv.
  *
  * The reference is pure R (DESCRIPTION: "NeedsCompilation: no"; NAMESPACE has no useDynLib), so it

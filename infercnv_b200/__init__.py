@@ -1,4 +1,4 @@
-"""infercnv_b200 - B200 (sm_100a) engine for inferCNV's smoothing + HMM hot path.
+"""infercnv_b200 - H100 (sm_90a) engine for inferCNV's smoothing + HMM hot path.
 
 The product is `libinfercnv_b200.so` (C ABI in include/infercnv_b200.h, CUDA in csrc/).
 The Python around it is plumbing:

@@ -1,7 +1,7 @@
 """NumPy-facing wrappers of the host-pointer C ABI (the same entry points the R shim binds).
 
 Matrices are (G genes, C cells) float64, Fortran order (R column-major: a cell's genes are
-contiguous).  Indices are 0-based.  Every call goes H2D -> sm_100a kernels -> D2H inside the
+contiguous).  Indices are 0-based.  Every call goes H2D -> sm_90a kernels -> D2H inside the
 library; nothing here computes on the CPU.
 """
 from __future__ import annotations

@@ -1,5 +1,5 @@
-"""Build libinfercnv_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the
-repo snapshot to the GPU box).  `python -m infercnv_b200.build [--force] [--verbose]`."""
+"""Build libinfercnv_b200.so in-tree with nvcc for sm_90a (no JIT cache: the .so is built once by
+__graft_entry__.build() and loaded from the tree).  `python -m infercnv_b200.build [--force] [--verbose]`."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libinfercnv_b200.so")
 SOURCES = ["icnv_api.cu", "icnv_smooth.cu", "icnv_viterbi.cu", "icnv_median_filter.cu", "icnv_reduce.cu",
            "icnv_synth.cu", "icnv_regions.cu", "icnv_ingest.cu", "icnv_dist.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def nvcc() -> str:

@@ -84,8 +84,7 @@ int device_slots() { return g_slots; }
 // the caller's slab into / out of them at memory bandwidth, so PCIe sees pinned transfers only.
 // One thread's share of a staging copy, with NON-TEMPORAL stores: the destination (a pinned ring slot the DMA engine reads
 // next, or the caller's result matrix) is not read again by this thread, so writing around the cache saves the write-allocate
-// read of every line - glibc's memcpy only does that above ~3/4 of the last-level cache per call, which is why the
-// end-to-end time dropped by 18 % between 2048- and 4096-cell slabs before this (profiles/r02_e2e_probe.txt).
+// read of every line - glibc's memcpy only does that above ~3/4 of the last-level cache per call.
 static void stream_copy(char *d, const char *s, size_t n) {
 #if defined(__x86_64__) && defined(__SSE2__)
     if (n < (size_t)1 << 16) {
@@ -400,8 +399,8 @@ static int init_slot(int slot, int device) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) return set_error(ICNV_E_NO_DEVICE, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major < 10)
-        return set_error(ICNV_E_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0)
+        return set_error(ICNV_E_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device,
                          prop.major, prop.minor);
     c.sm_count = prop.multiProcessorCount;
     c.smem_optin = (int)prop.sharedMemPerBlockOptin;
@@ -496,7 +495,7 @@ void icnv_shutdown(void) {
 }
 
 const char *icnv_last_error(void) { return g_err; }
-const char *icnv_version(void) { return "infercnv_b200 0.1.0 (sm_100a)"; }
+const char *icnv_version(void) { return "infercnv_b200 0.1.0 (sm_90a)"; }
 int64_t icnv_launch_count(void) {
     int64_t n = 0;
     for (int s = 0; s < std::max(1, g_slots); ++s) n += g_ctx[s].launches.load();
@@ -696,8 +695,7 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     int64_t slab_cells = hmm ? SLAB_CELLS : SLAB_CELLS_SMOOTH;
     if (stage_in || stage_out) {
         // pageable caller memory: fewer, larger hand-overs to the copy threads - about 320 MB of input per slab (4000 cells at
-        // 10 000 genes: 362 ms against 386 ms with 1024-cell slabs for c3, profiles/r02_e2e_probe.txt), but at least ten slabs
-        // so that filling and draining the pipeline stays a small share
+        // 10 000 genes), but at least ten slabs so that filling and draining the pipeline stays a small share
         int64_t by_bytes = ((int64_t)(320e6 / (8.0 * (double)G)) + 31) / 32 * 32;
         by_bytes = std::max<int64_t>(256, std::min<int64_t>(8192, by_bytes));
         const int64_t by_count = std::max<int64_t>(SLAB_CELLS, ((C + 9) / 10 + 31) / 32 * 32);

@@ -1,5 +1,5 @@
 // icnv_common.cuh - context, error plumbing and small device helpers shared by the kernels of
-// libinfercnv_b200.so (sm_100a only).
+// libinfercnv_b200.so (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

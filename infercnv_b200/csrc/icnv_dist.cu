@@ -8,7 +8,7 @@
 // The sum is taken in the DIFFERENCE form, gene by gene in gene order, one fused multiply-add per term: no |a|^2 + |b|^2 -
 // 2 a.b cancellation, so near-identical cells (which hclust merges first) keep full relative accuracy.  That form is two
 // FP64 instructions per (pair, gene) and nothing else matters: the kernel is bound by the FP64 pipe (64 lanes per clock per
-// SM on B200, the same rate its FP64 tensor path has), not by HBM - a 128 x 128 tile of pairs re-uses every value it loads
+// SM on H100; its FP64 tensor path is twice that, but only for the cancelling a.b form), not by HBM - a 128 x 128 tile of pairs re-uses every value it loads
 // 128 times from shared memory.
 //
 // One CTA = one 128 x 128 tile of the upper triangle (tiles below the diagonal exit at once), 256 threads, 8 x 8 pairs per

@@ -70,8 +70,8 @@ __global__ void __launch_bounds__(RG_CT) state_counts_kernel(const uint8_t *__re
         pending = 0;
     };
     // eight listed cells per round: their (index, state word) loads are issued back to back before any of them is
-    // used - one cell at a time the loop is a chain of two dependent loads per 4 bytes and ran at 0.05 of the HBM
-    // roofline (profiles/r01b_secondary_kernels.json).  Past the chunk's end the last cell is re-read and not counted.
+    // used - one cell at a time the loop is a chain of two dependent loads per 4 bytes.  Past the chunk's end the last
+    // cell is re-read and not counted.
     constexpr int RG_BATCH = 8;
     const bool whole_word = ALIGNED && g0 + RG_GPT <= G;
     for (int i = ch.begin; i < ch.end; i += RG_BATCH) {

@@ -1,4 +1,4 @@
-// icnv_smooth.cu - the smooth block of infercnv::run() as sm_100a kernels.
+// icnv_smooth.cu - the smooth block of infercnv::run() as sm_90a kernels.
 //
 //   K1  group_partial_sums / combine_partials / bounds_from_means
 //         .get_normal_gene_mean_bounds (R/inferCNV_ops.R:1708-1735): per-gene mean over each
@@ -12,7 +12,7 @@
 //
 // Data layout: X[g + ld*c], a cell's genes contiguous (R column-major).  HBM-bound integer-free
 // streaming work: no tensor cores; what matters is coalesced 8/16-byte accesses, the column kept
-// on chip between the stages, and a grid that fills 148 SMs x resident CTAs.
+// on chip between the stages, and a grid that fills the SMs (132 on an H100) x resident CTAs.
 #include <cfloat>
 #include <cmath>
 #include <cstring>
@@ -334,7 +334,7 @@ __device__ __forceinline__ double fast_exp2_nc(double x, const double *__restric
 // dead-band subtraction, .subtract_expr (ops.R:1764-1769): strict inequalities
 __device__ __forceinline__ double sub_bounds(double x, double lo, double hi) {
     // x-hi above the band, x-lo below it, exactly 0 inside (lo <= hi always).  Written with compares and selects:
-    // double-precision fmin / fmax expand to ~17 instructions each on sm_100, this form is 8 in total.
+    // double-precision fmin / fmax carry NaN handling this comparison does not need.
     const double above = x - hi, below = x - lo;
     return (x > hi) ? above : ((x < lo) ? below : 0.0);
 }
@@ -1803,10 +1803,7 @@ int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx, const in
     // ---- v4 (single padded buffer, stages in place): columns too long for v3's two buffers (> ~12 400 genes at window
     // 101; config c5's 20 000 genes run here, one 1024-thread CTA per SM), or everywhere with ICNV_CELL_KERNEL=4 (read at
     // icnv_init): two 512-thread CTAs per SM when a CTA's buffer allows it, four 256-thread CTAs for small columns.
-    // Measured at 10 000 genes (profiles/r02_*): v4 with two cells per SM 1.21 ms per 9 000 cells against v3's 1.14 ms -
-    // its chunk-descriptor loops cost more instructions than the second cell in flight wins back - so v3 stays the default
-    // where it fits; at 20 000 genes v4 runs 62 500 cells in 13.8 ms where the register-resident v2 kernel it replaced
-    // took 25.4 ms.
+    // v3 stays the default where it fits; DESIGN.md section 3 K2 has the H100 measurements of both at 10 000 genes.
     {
         const int pad = 2 * h + 2;
         std::vector<Chr4> chr((size_t)K + 1);

@@ -1,4 +1,4 @@
-// icnv_viterbi.cu - K3: the i6 / i3 HMM of inferCNV as an sm_100a kernel.
+// icnv_viterbi.cu - K3: the i6 / i3 HMM of inferCNV as an sm_90a kernel.
 //
 // Restates Viterbi.dthmm.adj (R/inferCNV_HMM.R:1101-1176) for every (cell-or-group, chromosome)
 // sequence at once.  One thread owns one sequence; the 32 lanes of a warp are 32 consecutive
@@ -7,7 +7,7 @@
 // mean / log Pi / log delta sit in the kernel-parameter constant bank (warp-uniform operands).
 // Backpointers (3 bits per state, one 32-bit word per gene) go to a per-warp scratch ring laid out
 // [gene][lane], i.e. one coalesced 128-byte line per gene, sized for the longest chromosome and
-// re-used for every work item, so it stays resident in the 126 MB L2.
+// re-used for every work item, so its lines are written to and read back from L2.
 //
 // Arithmetic: "exact" mode follows the reference's operation order in IEEE double without FMA
 // contraction (explicit __dmul_rn/__dadd_rn/__ddiv_rn), including nmath's pnorm_both
@@ -333,10 +333,8 @@ constexpr int FAST_WARPS = 16;   // default warps per CTA (one CTA per SM: the r
                                  // the gene loop stays spill-free, ~19 values are re-loaded from local memory per 8-gene tile
 constexpr int TAB_REP = 8;       // table replicas: lane l reads replica l & 7, so a 16-byte lookup never bank-conflicts
 
-// L2 policies around the backpointer rings (129 MB at 16 warps x 148 SMs x 852 genes: more than the L2 holds beside the input
-// stream), measured at c3 (profiles/r02_hmm_fp32_cascade.md): no hint 13.2 GB of DRAM traffic per launch for 9 GB algorithmic;
-// input lines evict_first 16.7 GB (a 128-byte line holds two 8-gene tiles of a cell and is dropped between them) but 1 % faster;
-// ring stores evict_last 12.8 GB - the default; additionally discarding ring lines the trace-back has read 12.0 GB, 1 % slower.
+// L2 policies around the backpointer rings (16 warps x 132 SMs x the longest chromosome x 128 bytes: more than the 50 MB L2
+// of an H100 holds beside the input stream).  ICNV_VIT_EVICT selects one; DESIGN.md section 3 K3 has the measured choice.
 __device__ __forceinline__ unsigned long long l2_evict_first_policy(int evict_first) {
     unsigned long long pol;
     if (evict_first) asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -1098,7 +1096,7 @@ int icnv_dev_scatter_group_states_u8(const uint8_t *gs, int64_t G, int64_t C, co
     ICNV_REQUIRE_READY();
     if (!gs || !grp_of || !out || G <= 0 || C <= 0) return set_error(ICNV_E_BAD_ARG, "icnv_dev_scatter_group_states_u8: bad argument");
     int64_t blocks = (G * C + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (int64_t)ctx().sm_count * 32) blocks = (int64_t)ctx().sm_count * 32;
     scatter_group_states_u8_kernel<<<(unsigned)blocks, 256, 0, pick_stream(stream)>>>(gs, G, C, grp_of, out);
     ICNV_CHECK_LAUNCH("scatter_group_states_u8_kernel");
     return ICNV_OK;
@@ -1107,7 +1105,7 @@ int icnv_dev_scatter_group_states_u8(const uint8_t *gs, int64_t G, int64_t C, co
 int icnv_dev_widen_states(const uint8_t *s, int32_t *out, int64_t n, void *stream) {
     ICNV_REQUIRE_READY();
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (int64_t)ctx().sm_count * 32) blocks = (int64_t)ctx().sm_count * 32;
     widen_states_kernel<<<(unsigned)blocks, 256, 0, pick_stream(stream)>>>(s, out, n);
     ICNV_CHECK_LAUNCH("widen_states_kernel");
     return ICNV_OK;
@@ -1116,7 +1114,7 @@ int icnv_dev_widen_states(const uint8_t *s, int32_t *out, int64_t n, void *strea
 int icnv_dev_narrow_states(const int32_t *s, uint8_t *out, int64_t n, void *stream) {
     ICNV_REQUIRE_READY();
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (int64_t)ctx().sm_count * 32) blocks = (int64_t)ctx().sm_count * 32;
     narrow_states_kernel<<<(unsigned)blocks, 256, 0, pick_stream(stream)>>>(s, out, n);
     ICNV_CHECK_LAUNCH("narrow_states_kernel");
     return ICNV_OK;
@@ -1126,7 +1124,7 @@ int icnv_dev_scatter_group_states(const uint8_t *gs, int64_t G, int64_t C, const
                                   void *stream) {
     ICNV_REQUIRE_READY();
     int64_t blocks = (G * C + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > (int64_t)ctx().sm_count * 32) blocks = (int64_t)ctx().sm_count * 32;
     scatter_group_states_kernel<<<(unsigned)blocks, 256, 0, pick_stream(stream)>>>(gs, G, C, grp_of, out);
     ICNV_CHECK_LAUNCH("scatter_group_states_kernel");
     return ICNV_OK;

@@ -1,6 +1,6 @@
 ## infercnv_b200.R - drop-in GPU replacements for inferCNV's smoothing + HMM hot path.
 ##
-## Usage (on a box with R, the infercnv package and a B200):
+## Usage (on a box with R, the infercnv package and an H100):
 ##   R CMD SHLIB infercnvb200_shim.c -I<repo>/include -L<repo>/infercnv_b200 -linfercnv_b200
 ##   dyn.load("<repo>/infercnv_b200/libinfercnv_b200.so"); dyn.load("infercnvb200_shim.so")
 ##   source("infercnv_b200.R"); infercnvb200_install()
@@ -77,7 +77,7 @@ b200_subtract_ref_expr_from_obs <- function(infercnv_obj, inv_log=FALSE, use_bou
     orig <- .icnv_env$orig$subtract_ref_expr_from_obs
     m <- infercnv_obj@expr.data
     if (!.icnv_enabled() || !.icnv_ok(m)) return(orig(infercnv_obj, inv_log=inv_log, use_bounds=use_bounds))
-    futile.logger::flog.info(sprintf("::subtract_ref_expr_from_obs:Start inv_log=%s, use_bounds=%s (B200)", inv_log, use_bounds))
+    futile.logger::flog.info(sprintf("::subtract_ref_expr_from_obs:Start inv_log=%s, use_bounds=%s (GPU)", inv_log, use_bounds))
     res <- tryCatch(.Call("icnvR_subtract_ref", m, .icnv_ref_groups(infercnv_obj), inv_log, use_bounds), "available")
     if (is.null(res)) return(orig(infercnv_obj, inv_log=inv_log, use_bounds=use_bounds))
     infercnv_obj@expr.data <- .icnv_keep_names(res, m)
@@ -111,7 +111,7 @@ b200_center_cell_expr_across_chromosome <- function(infercnv_obj, method="mean")
     orig <- .icnv_env$orig$center_cell_expr_across_chromosome
     m <- infercnv_obj@expr.data
     if (!.icnv_enabled() || !.icnv_ok(m)) return(orig(infercnv_obj, method))
-    futile.logger::flog.info("::center_smooth across chromosomes per cell (B200)")
+    futile.logger::flog.info("::center_smooth across chromosomes per cell (GPU)")
     res <- .icnv_try(.Call("icnvR_center", m, identical(method, "median")), "center")
     if (is.null(res)) return(orig(infercnv_obj, method))
     infercnv_obj@expr.data <- .icnv_keep_names(res, m)
@@ -244,7 +244,7 @@ b200_normalize_counts_by_seq_depth <- function(infercnv_obj, normalize_factor=NA
         ## sparse counts (R/inferCNV.R:158-160): the compressed columns cross PCIe, the dense normalised matrix comes back
         res <- .icnv_try(.Call("icnvR_csc_normalize", m@p, m@i, as.double(m@x), dim(m), as.double(normalize_factor)), "csc_normalize")
         if (!is.null(res)) {
-            futile.logger::flog.info("normalizing counts matrix by depth (B200, sparse input)")
+            futile.logger::flog.info("normalizing counts matrix by depth (GPU, sparse input)")
             infercnv_obj@expr.data <- .icnv_keep_names(res, m)
             return(infercnv_obj)
         }
@@ -278,7 +278,7 @@ b200_predict_CNV_via_HMM_on_tumor_subclusters_per_chr <- function(infercnv_obj, 
     codes <- .icnv_chr_codes(infercnv_obj)
     if (is.null(subclusters_per_chr) || !.icnv_enabled() || !.icnv_ok(m) || is.null(codes))
         return(orig(infercnv_obj, subclusters_per_chr, cnv_mean_sd, cnv_level_to_mean_sd_fit, t))
-    futile.logger::flog.info("predict_CNV_via_HMM_on_tumor_subclusters_per_chr (B200)")
+    futile.logger::flog.info("predict_CNV_via_HMM_on_tumor_subclusters_per_chr (GPU)")
     chrs <- unique(infercnv_obj@gene_order$chr)
     per <- lapply(chrs, function(chr) lapply(subclusters_per_chr[[chr]], as.integer))
     flat <- unlist(per, recursive=FALSE)
@@ -299,7 +299,7 @@ b200_scale_infercnv_expr <- function(infercnv_obj) {
     orig <- .icnv_env$orig$scale_infercnv_expr
     m <- infercnv_obj@expr.data
     if (!.icnv_enabled() || !.icnv_ok(m)) return(orig(infercnv_obj))
-    futile.logger::flog.info("-scaling expr data (B200)")
+    futile.logger::flog.info("-scaling expr data (GPU)")
     res <- .icnv_try(.Call("icnvR_scale", m), "scale")
     if (is.null(res)) return(orig(infercnv_obj))
     infercnv_obj@expr.data <- .icnv_keep_names(res, m)
@@ -318,7 +318,7 @@ b200_remove_outliers_norm <- function(infercnv_obj, out_method="average_bound", 
     ## anything but hard bounds / "average_bound" ends in the reference's stop(991) / stop(992): leave it to R
     if (!.icnv_enabled() || !.icnv_ok(m) || !(hard || identical(out_method, "average_bound")))
         return(orig(infercnv_obj, out_method, lower_bound, upper_bound))
-    futile.logger::flog.info(paste("::remove_outlier_norm:Start (B200)", "out_method:", out_method, "lower_bound:", lower_bound,
+    futile.logger::flog.info(paste("::remove_outlier_norm:Start (GPU)", "out_method:", out_method, "lower_bound:", lower_bound,
                                    "upper_bound:", upper_bound))
     res <- .icnv_try(.Call("icnvR_remove_outliers", m, as.double(if (hard) lower_bound else NA),
                           as.double(if (hard) upper_bound else NA)), "remove_outliers")
@@ -355,7 +355,7 @@ b200_get_predicted_CNV_regions <- function(infercnv_obj, by=c("consensus", "subc
     codes <- .icnv_chr_codes(infercnv_obj)
     go <- infercnv_obj@gene_order
     if (!.icnv_enabled() || !.icnv_ok(m) || is.null(codes) || anyNA(go$start) || anyNA(go$stop)) return(orig(infercnv_obj, by))
-    futile.logger::flog.info(sprintf("get_predicted_CNV_regions(%s) (B200)", by))
+    futile.logger::flog.info(sprintf("get_predicted_CNV_regions(%s) (GPU)", by))
     if (is.null(infercnv_obj@tumor_subclusters)) {
         futile.logger::flog.warn("get_predicted_CNV_regions() - no subclusters defined, resetting reporting mode to consensus")
         by <- "consensus"
@@ -409,7 +409,7 @@ infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_c
     codes <- .icnv_chr_codes(infercnv_obj)
     if (!.icnv_enabled() || !.icnv_ok(m) || is.null(codes) || window_length < 2 || window_length %% 2 == 0 ||
         is.na(max_centered_threshold) || !is.numeric(max_centered_threshold)) return(NULL)
-    futile.logger::flog.info(sprintf("::smooth block (steps 4, 8-12, 14%s) in one pass (B200)", if (is.null(HMM_info)) "" else " + per-cell HMM"))
+    futile.logger::flog.info(sprintf("::smooth block (steps 4, 8-12, 14%s) in one pass (GPU)", if (is.null(HMM_info)) "" else " + per-cell HMM"))
     refs <- .icnv_ref_groups(infercnv_obj)
     hmm_obj <- NULL
     if (is.null(HMM_info)) {

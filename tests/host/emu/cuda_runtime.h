@@ -83,7 +83,7 @@ struct cudaDeviceProp {
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) {
-    p->major = 10; p->minor = 0; p->multiProcessorCount = 4; p->sharedMemPerBlockOptin = 227 * 1024;
+    p->major = 9; p->minor = 0; p->multiProcessorCount = 4; p->sharedMemPerBlockOptin = 227 * 1024;
     return cudaSuccess;
 }
 static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { *s = (cudaStream_t)malloc(8); return cudaSuccess; }

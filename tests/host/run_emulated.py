@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""TEST INFRASTRUCTURE: run the GPU parity tests (the same test functions the B200 box runs with -m gpu) against
+"""TEST INFRASTRUCTURE: run the GPU parity tests (the same test functions an H100 runs with -m gpu) against
 tests/host/_build/libinfercnv_b200_emu.so, i.e. against the kernels' own source text executed by the host emulation of
 the CUDA execution model in tests/host/emu/cuda_runtime.h.  A separate process, because it points the ctypes loader at
 the emulated library before anything is loaded; the package itself has no such switch.

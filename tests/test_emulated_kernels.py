@@ -3,7 +3,7 @@ translation unit of infercnv_b200/csrc with g++ against a host emulation of the 
 (tests/host/emu/cuda_runtime.h: the threads of a block are fibers; __syncthreads, warp shuffles / reductions and atomics
 have their CUDA semantics; a divergent barrier or a live-lock aborts; fresh device and shared memory is poisoned), with
 synchronous stand-ins for the few inline-PTX copy primitives (TMA bulk copy + mbarrier, cp.async), and
-tests/host/run_emulated.py runs the SAME parity tests the B200 box runs (-m gpu) against that build in a subprocess.
+tests/host/run_emulated.py runs the SAME parity tests an H100 runs (-m gpu) against that build in a subprocess.
 
 Test infrastructure only: it exercises the kernels' index arithmetic, barriers, shared-memory hand-offs and memory
 accesses without a GPU - the fused cell pipeline, both Viterbi kernels with the certificate / re-run logic, the median

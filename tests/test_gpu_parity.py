@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C ABI) against the CPU oracle and the reference's own
-known answers.  Needs a B200: run with `pytest -m gpu`.
+known answers.  Needs an H100: run with `pytest -m gpu`.
 
 Tolerances (BASELINE.json north_star): smoothed matrix within 1e-5 relative; HMM state calls
 bit-identical.  The smooth tests additionally report how far below that the kernels actually are.

@@ -59,9 +59,9 @@ D = torch.empty(n_d * (n_d - 1) // 2, dtype=torch.float64, device=Y.device)
 cells_d = np.arange(1000, 1000 + n_d, dtype=np.int32)   # the observation cells of the c2 matrix
 ms = timed(lambda: eng.pairwise_dist(Y, cells_d, out=D))
 pair_genes = n_d * (n_d - 1) / 2 * G
-sm_mhz = float(torch.cuda.clock_rate()) if hasattr(torch.cuda, "clock_rate") else 1965.0
+sm_mhz = float(torch.cuda.clock_rate()) if hasattr(torch.cuda, "clock_rate") else 1980.0
 out["pairwise_dist_9000_cells"] = {"ms": ms, "pair_genes_per_s": pair_genes / ms * 1e3, "fp64_instr_per_s": 2 * pair_genes / ms * 1e3,
-                                   "fp64_pipe_frac_at_64_per_clk_per_sm": 2 * pair_genes / (ms * 1e-3) / (64 * 148 * sm_mhz * 1e6),
+                                   "fp64_pipe_frac_at_64_per_clk_per_sm": 2 * pair_genes / (ms * 1e-3) / (64 * torch.cuda.get_device_properties(0).multi_processor_count * sm_mhz * 1e6),
                                    "tiles_computed": ((n_d + 127) // 128) * ((n_d + 127) // 128 + 1) // 2,
                                    "sm_mhz": sm_mhz}
 # ---- region calling on the device-resident i6 states (K7), ingest (K8) and the element-wise steps (K9) ----

@@ -145,7 +145,7 @@ def emit(name, ops, ins, outs, in_names, out_name, doc):
 
 def main():
     parts = ["// icnv_median_merge.inc - generated by tools/gen_median_merge.py; do not edit.  See that file for what the networks are.",
-             "// mf_min / mf_max are defined by the includer (unsigned min / max: VIMNMX.U32 on sm_100a)."]
+             "// mf_min / mf_max are defined by the includer (unsigned min / max: VIMNMX.U32 on sm_90a)."]
     ops, ins, outs = build_sort9()
     # sort9 works in place on one array: emit as input k, output k
     parts.append(emit("MF_SORT9", ops, ins, outs, ["k_"], "r_", "sort 9 keys (25 comparators, 7 layers)"))

@@ -1,5 +1,5 @@
-// Issue rate of the min/max flavours a comparator network can be built from (sm_100a): which pipe, how many per clock.
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o /tmp/minmax_rate tools/microbench/minmax_rate.cu && /tmp/minmax_rate
+// Issue rate of the min/max flavours a comparator network can be built from (sm_90a): which pipe, how many per clock.
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/microbench/minmax_rate.bin tools/microbench/minmax_rate.cu && tools/microbench/minmax_rate.bin
 #include <cstdio>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -35,23 +35,25 @@ __global__ void __launch_bounds__(256) k(unsigned *out, int iters) {
 template <int MODE>
 void run(const char *name) {
     unsigned *d;
-    cudaMalloc(&d, 148 * 8 * 256 * sizeof(unsigned));
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&d, sms * 8 * 256 * sizeof(unsigned));
     const int iters = 20000;
-    k<MODE><<<148 * 8, 256>>>(d, 100);
+    k<MODE><<<sms * 8, 256>>>(d, 100);
     cudaDeviceSynchronize();
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a);
-    k<MODE><<<148 * 8, 256>>>(d, iters);
+    k<MODE><<<sms * 8, 256>>>(d, iters);
     cudaEventRecord(b);
     cudaEventSynchronize(b);
     float ms;
     cudaEventElapsedTime(&ms, a, b);
-    const double ops = 148.0 * 8 * 256 * (double)iters * 8 * 2;   // min + max per pair
+    const double ops = (double)sms * 8 * 256 * (double)iters * 8 * 2;   // min + max per pair
     int clk = 0;
     cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
     printf("%-14s %8.3f ms  %7.2f Gop/s  = %5.1f min/max per clock per SM (+ 0.5 IADD each) at %d MHz\n", name, ms, ops / ms / 1e6,
-           ops / (ms * 1e-3) / 148.0 / (clk * 1e3), clk / 1000);
+           ops / (ms * 1e-3) / sms / (clk * 1e3), clk / 1000);
     cudaFree(d);
 }
 

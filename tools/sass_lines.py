@@ -3,7 +3,7 @@
 
     python tools/sass_lines.py icnv_smooth.cu cell_pipeline3_kernelILi1024 [--lines A:B] [--ops]
 
-Compiles csrc/<file> to a cubin for sm_100a with -lineinfo, disassembles it with `nvdisasm -g -c` and attributes
+Compiles csrc/<file> to a cubin for sm_90a with -lineinfo, disassembles it with `nvdisasm -g -c` and attributes
 every instruction of the kernel whose mangled name contains the pattern to the source line of the preceding
 line marker.  Prints instructions per source line (with the source text) and per opcode class: the instruction
 count of a loop body is the number the issue-bound kernels (DESIGN.md K2 / K3) are tuned against before a GPU
@@ -51,7 +51,7 @@ def main():
     with tempfile.TemporaryDirectory() as td:
         cubin = os.path.join(td, "k.cubin")
         subprocess.check_call(["nvcc", "-ccbin", "/usr/bin/g++", "-O3", "-std=c++17", "-lineinfo", "-gencode",
-                               "arch=compute_100a,code=sm_100a", "-cubin", src, "-o", cubin], stderr=subprocess.DEVNULL)
+                               "arch=compute_90a,code=sm_90a", "-cubin", src, "-o", cubin], stderr=subprocess.DEVNULL)
         dis = subprocess.run(["nvdisasm", "-g", "-c", cubin], capture_output=True, text=True).stdout
     text = open(src).read().split("\n")
     lo, hi = (int(v) for v in a.lines.split(":")) if a.lines else (0, 10 ** 9)
