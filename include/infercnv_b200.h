@@ -374,6 +374,11 @@ ICNV_API int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx,
                                         const double *hi1, const double *mid1, double threshold, int window,
                                         int center, const double *lo2, const double *hi2, const double *mid2,
                                         int apply_exp2, int *err_flag, void *stream);
+/* Which instantiation of the fused kernel the last icnv_dev_cell_pipeline_f64 call on this device launched (read-only;
+ * the host entry points go through it too): out6 = {family (3: two-buffer kernel, 4: single-buffer kernel), threads per
+ * CTA, minimum CTAs per SM of its launch bounds, padded-Q layout (0 / 1), fully unrolled slice length (0: generic loops),
+ * slice length L of the segment table}.  All zero when that call launched nothing (refused, or no columns). */
+ICNV_API int icnv_debug_cell_kernel(int *out6);
 
 /* Whole smooth block on device-resident data (single GPU): X, Y are G x C (ld = G). */
 ICNV_API int icnv_dev_smooth_block_f64(const double *X, double *Y, int64_t G, int64_t C,

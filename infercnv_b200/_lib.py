@@ -61,6 +61,7 @@ SIGNATURES = {
     "icnv_dev_bounds_from_means_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P, _P]),
     "icnv_dev_cell_pipeline_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, _P, c_i64, _P, _P, c_int, c_int, _P, _P, _P,
                                            ct.c_double, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
+    "icnv_debug_cell_kernel": (c_int, [_P]),
     "icnv_dev_smooth_block_f64": (c_int, [_P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,
                                           c_int, c_int, _P]),
     "icnv_dev_viterbi_f64": (c_int, [_P, c_i64, c_i64, _P, _P, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, _P]),

@@ -92,6 +92,14 @@ def set_hmm_mode(mode) -> None:
     _lib.check(_lib.load().icnv_set_hmm_mode(int(m)))
 
 
+def last_cell_kernel() -> tuple:
+    """(family, NT, MINB, PADQ, LFIX, L) of the fused cell-pipeline instantiation the last smooth-block / cell-pipeline call
+    launched (icnv_debug_cell_kernel); all zero when it launched nothing."""
+    out = (ct.c_int * 6)()
+    _lib.check(_lib.load().icnv_debug_cell_kernel(ct.addressof(out)))
+    return tuple(int(v) for v in out)
+
+
 def hmm_rerun_count() -> int:
     return int(_lib.load().icnv_hmm_rerun_count())
 

@@ -85,6 +85,9 @@ struct Ctx {
     int opt_cell_kernel = 0, opt_cell_nt = 0, opt_cell_variant = -1, opt_cell_padq = 1, opt_cell_lfix = 1;
     int opt_vfast_warps = 0, opt_mf_kernel = -1, opt_mf_list32 = 0, opt_vit_evict = 2;
     long opt_slab_cells = 0;
+    // the cell-pipeline instantiation the last icnv_dev_cell_pipeline_f64 call launched: family (3 / 4), NT, MINB, PADQ, LFIX,
+    // slice length L; all zero when that call launched nothing (refused, or no columns)
+    int cell_kernel[6] = {};
     std::mutex mu;
 };
 

@@ -1211,7 +1211,9 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
     double *cand = tails + 2 * NW;
     Red<NW> &red = *reinterpret_cast<Red<NW> *>(cand + CAND_MAX + 2);
     unsigned long long *bar = reinterpret_cast<unsigned long long *>(&red + 1);
-    int4 *ctab = reinterpret_cast<int4 *>(bar + 2);           // [n_chunks] chunk descriptors
+    // [n_chunks] chunk descriptors, read as 16-byte int4: rounded up to a 16-byte boundary (bar + 2 sits 8 bytes off one
+    // whenever h is odd - the offsets in front of it are h + 2 plus even counts of doubles)
+    int4 *ctab = reinterpret_cast<int4 *>((reinterpret_cast<uintptr_t>(bar + 2) + 15) & ~(uintptr_t)15);
     int *hist = reinterpret_cast<int *>(ctab + p.n_chunks);   // NB bins, zero between cells
     int *hres = hist + NB;
     int *wcnt = hres + 8;                                     // [2][NW]
@@ -1709,6 +1711,13 @@ ICNV_API int icnv_debug_stats(unsigned long long *out4, int reset) {
     return ICNV_OK;
 }
 
+ICNV_API int icnv_debug_cell_kernel(int *out6) {
+    ICNV_REQUIRE_READY();
+    if (!out6) return set_error(ICNV_E_BAD_ARG, "icnv_debug_cell_kernel: out6 is NULL");
+    std::copy(ctx().cell_kernel, ctx().cell_kernel + 6, out6);
+    return ICNV_OK;
+}
+
 int icnv_dev_invlog_finish_f64(double *means, int64_t n, void *stream) {
     ICNV_REQUIRE_READY();
     invlog_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, pick_stream(stream)>>>(means, n);
@@ -1723,6 +1732,7 @@ int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx, const in
                                int *err_flag, void *stream) {
     ICNV_REQUIRE_READY();
     Ctx &c = ctx();
+    for (int &v : c.cell_kernel) v = 0;
     if (!X || !Y || G <= 0 || n_cols < 0 || ldx < G || ldy < G || !chr_start || !chr_len || K <= 0)
         return set_error(ICNV_E_BAD_ARG, "icnv_dev_cell_pipeline_f64: bad argument");
     if ((lo1 == nullptr) != (hi1 == nullptr) || (lo2 == nullptr) != (hi2 == nullptr))
@@ -1795,6 +1805,8 @@ int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx, const in
                 rc3 = (nt3 == 256) ? launch3(cell_pipeline3_kernel<256, false, 0>)
                                    : (nt3 == 512 ? launch3(cell_pipeline3_kernel<512, false, 0>) : launch3(cell_pipeline3_kernel<1024, false, 0>));
             if (rc3) return rc3;
+            const int sel3[6] = {3, nt3, 1, padq, lfix, L3};
+            std::copy(sel3, sel3 + 6, c.cell_kernel);
             ICNV_CHECK_LAUNCH("cell_pipeline3_kernel");
             return ICNV_OK;
         }
@@ -1834,7 +1846,7 @@ int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx, const in
         auto smem4 = [&](int nt) {
             const int nw = nt / 32;
             const size_t red = (nt == 256) ? sizeof(Red<8>) : (nt == 512 ? sizeof(Red<16>) : sizeof(Red<32>));
-            return 128 * 24 + sizeof(double) * ((size_t)nb + (size_t)(h + 2) + 2 * (size_t)K + 2 * (size_t)nw + CAND_MAX + 2) + red + 16 +
+            return 128 * 24 + sizeof(double) * ((size_t)nb + (size_t)(h + 2) + 2 * (size_t)K + 2 * (size_t)nw + CAND_MAX + 2) + red + 16 + 8 +
                    sizeof(int) * (1024 + 8 + 2 * (size_t)nw + 2 + 32) + sizeof(Chr4) * ((size_t)K + 1) + sizeof(int4) * (size_t)nch + 16;
         };
         const size_t sm_total = 228 * 1024;     // shared memory of an SM; every resident CTA also reserves 1 KB
@@ -1889,6 +1901,10 @@ int icnv_dev_cell_pipeline_f64(const double *X, int64_t G, int64_t ldx, const in
             else if (nt4 == 512) rc4 = launch4(cell_pipeline4_kernel<512, 1, 1024, 0>);
             else rc4 = fix21 ? launch4(cell_pipeline4_kernel<1024, 1, 1024, 21>) : launch4(cell_pipeline4_kernel<1024, 1, 1024, 0>);
             if (rc4) return rc4;
+            const int minb4 = nt4 == 256 ? (minb >= 4 ? 4 : 1) : (nt4 == 512 ? (minb >= 2 ? 2 : 1) : 1);
+            const int lfix4 = (fix21 && (nt4 == 1024 || minb4 == 2)) ? 21 : 0;   // the instantiations with unrolled scans
+            const int sel4[6] = {4, nt4, minb4, 0, lfix4, L4};
+            std::copy(sel4, sel4 + 6, c.cell_kernel);
             ICNV_CHECK_LAUNCH("cell_pipeline4_kernel");
             return ICNV_OK;
         }

@@ -27,15 +27,19 @@ EMULATED = ["icnv_api.cu", "icnv_regions.cu", "icnv_ingest.cu", "icnv_reduce.cu"
 
 # The asynchronous-copy primitives (inline PTX) get synchronous stand-ins: the copy happens when it is issued - the
 # earliest moment the hardware could perform it, so a buffer that is still being read when its refill is issued shows
-# up as wrong results.  An mbarrier is emulated as a count of completed phases; a thread waiting for a phase that is not
-# complete yet yields to the other threads of the block (the issuing thread may not have run yet), and a block in
-# which everybody only waits is reported as a dead-lock.
+# up as wrong results.  An mbarrier is emulated as a count of completed phases plus, in the word behind it, the transaction
+# bytes announced by expect_tx and not yet delivered: a phase completes only when every announced byte has been copied
+# (emu::tx_complete_check), and every bulk copy obeys cp.async.bulk's 16-byte alignment and size rule
+# (emu::bulk_copy_check) - the two ways a wrong byte count or frame offset would hang or corrupt the GPU's copy.  A thread
+# waiting for a phase that is not complete yet yields to the other threads of the block (the issuing thread may not have
+# run yet), and a block in which everybody only waits is reported as a dead-lock.
 PTX_STANDINS = {
-    "mbar_init": "{ (void)count; *reinterpret_cast<unsigned long long *>(bar) = 0ull; }",
-    "mbar_expect_tx": "{ (void)bar; (void)bytes; }",
-    "bulk_g2s": "{ memcpy(dst, src, bytes); *reinterpret_cast<unsigned long long *>(bar) += 1ull; }",
-    "bulk_g2s_multi": "{ memcpy(dst, src, bytes); (void)bar; }",
-    "mbar_host_commit": "{ *reinterpret_cast<unsigned long long *>(bar) += 1ull; }",
+    "mbar_init": "{ (void)count; reinterpret_cast<unsigned long long *>(bar)[0] = 0ull; reinterpret_cast<unsigned long long *>(bar)[1] = 0ull; }",
+    "mbar_expect_tx": "{ reinterpret_cast<unsigned long long *>(bar)[1] += bytes; }",
+    "bulk_g2s": "{ emu::bulk_copy_check(dst, src, bytes); memcpy(dst, src, bytes); unsigned long long *b = reinterpret_cast<unsigned long long *>(bar); "
+                "b[1] -= bytes; emu::tx_complete_check(b); b[0] += 1ull; }",
+    "bulk_g2s_multi": "{ emu::bulk_copy_check(dst, src, bytes); memcpy(dst, src, bytes); reinterpret_cast<unsigned long long *>(bar)[1] -= bytes; }",
+    "mbar_host_commit": "{ unsigned long long *b = reinterpret_cast<unsigned long long *>(bar); emu::tx_complete_check(b); b[0] += 1ull; }",
     "mbar_wait": "{ while (((*reinterpret_cast<volatile unsigned long long *>(bar)) & 1ull) == parity) emu::spin_yield(); }",
     "fence_proxy_async": "{ }",
     "cp_async8": "{ if (valid) memcpy(smem_dst, gsrc, 8); else memset(smem_dst, 0, 8); }",

@@ -190,6 +190,22 @@ inline void spin_yield() {
     cur->spun = true;
     yield_to_scheduler();
 }
+// The rules of cp.async.bulk and of the mbarrier's transaction count, for the synchronous stand-ins of
+// tests/host/build_emu.py: source and destination 16-byte aligned, a size that is a non-zero multiple of 16, and a phase
+// completed only when the bytes announced by expect_tx (kept in the word behind the phase word) have all arrived.  On the
+// GPU a short count leaves the barrier waiting forever and an excess completes the phase early; here both abort.
+inline void bulk_copy_check(const void *dst, const void *src, unsigned bytes) {
+    if (((uintptr_t)dst & 15u) || ((uintptr_t)src & 15u) || (bytes & 15u) || bytes == 0) {
+        fprintf(stderr, "emu: cp.async.bulk of %u bytes from %p to %p breaks the 16-byte alignment / size rule\n", bytes, src, dst);
+        abort();
+    }
+}
+inline void tx_complete_check(const unsigned long long *bar) {
+    if (bar[1] != 0ull) {
+        fprintf(stderr, "emu: mbarrier phase completed with %lld transaction bytes not matched by copies\n", (long long)bar[1]);
+        abort();
+    }
+}
 inline void trampoline() {
     (*body)();
     cur->state = DONE;

@@ -64,6 +64,21 @@ def single():
     Y_full, _ = eng.smooth_block(X, CS, LENS, refs)
     eng.reuse_reference_pass = True
     assert torch.equal(Y, Y_full)
+    # a strided view (column stride G + 1, G even): aligned columns take the bulk copy, the others the element-wise load,
+    # alternating inside each CTA's persistent loop and its prefetch of the next cell - same bits as the contiguous matrix
+    wide = torch.zeros((C, G + 1), dtype=torch.float64)
+    wide[:, :G] = X
+    assert G % 2 == 0 and wide[:, :G].stride(0) == G + 1
+    Y_wide, flag_w = eng.smooth_block(wide[:, :G], CS, LENS, refs)
+    assert torch.equal(Y_wide, Y) and int(flag_w.item()) == 0
+    b = tuple(torch.from_numpy(np.ascontiguousarray(v)) for v in (np.full(G, 0.2), np.full(G, 0.6), np.full(G, 0.4)))
+    cols = torch.from_numpy(np.array([69, 68, 3, 3, 0, 41, 0, 2], dtype=np.int32))     # pass 1's form: any order, repeats
+    outs = []
+    for Xin in (wide[:, :G], X):
+        Yc = torch.empty((len(cols), G), dtype=torch.float64)
+        eng.cell_pipeline(Xin, cols, Yc, CS, LENS, True, b, 3.0, 101, 1, b, True)
+        outs.append(Yc)
+    assert torch.equal(outs[0], outs[1])
     Y_scattered, _ = eng.smooth_block(X, CS, LENS, [np.array([3, 50, 7]), np.array([11, 60])])      # not leading: full pipeline
     want2 = orc.smooth_block(Xh, CS, LENS, [np.array([3, 50, 7]), np.array([11, 60])])
     assert float(np.max(np.abs(Y_scattered.numpy().T - want2) / np.abs(want2))) < 1e-11

@@ -36,6 +36,18 @@ def test_no_cpu_fallback_without_a_device():
     assert e.value.code == -1
     with pytest.raises(InfercnvB200Error):
         api.smooth_block(np.ones((6, 3)), [0], [6], [[0]])
+    with pytest.raises(InfercnvB200Error) as e:
+        api.last_cell_kernel()
+    assert e.value.code == -1
+
+
+def test_cell_kernel_query_is_declared_and_bound():
+    """icnv_debug_cell_kernel reports which fused cell-pipeline instantiation ran (tests/test_gpu_cell_pipeline_variants.py
+    asserts it per case): declared in the header, exported, six ints out."""
+    from infercnv_b200 import _lib
+    assert "icnv_debug_cell_kernel" in _declared()
+    assert _lib.SIGNATURES["icnv_debug_cell_kernel"] == (_lib.c_int, [_lib._P])
+    assert hasattr(_lib.load(), "icnv_debug_cell_kernel")
 
 
 def test_product_never_imports_the_oracle():
