@@ -20,6 +20,7 @@
 // of HBM traffic); see DESIGN.md for the roofline discussion.
 #include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <vector>
 #include <algorithm>
 
@@ -57,7 +58,11 @@ struct VitParams {
     const int32_t *chr_len_orig;
     // certified fast path
     double a_diag, b_off;      // log Pi diagonal / off-diagonal (all equal)
+    double cmove;              // a_diag - b_off: what moving costs against staying
+    int near_hi;               // high word of cmove - tau (the fast kernel's near-best check)
     double inv_sd;             // 1 / median sd
+    double emis_scale;         // 16 / sd and -mean_k * 16 / sd for the launch-wide sd (the fast kernel's table argument)
+    double emis_nms[MAXM];
     double tau;                // decision-margin threshold below which a sequence is re-run exactly
     const double *table;       // device copy of icnv_emis_table
     int means_monotone;        // state means sorted (either direction): the furthest state from any x is an end state
@@ -312,20 +317,26 @@ __global__ void __launch_bounds__(128) viterbi_kernel(const VitParams p) {
 //  (1) emission.  log(e_k / sum_j e_j) = g(z_k) - log(sum_j e_j) with g(z) = -log(-log Q(z)).  The
 //      second term is the same for every state of a gene, so it shifts all path scores equally and
 //      no arg-max sees it: it is dropped.  g comes from a piecewise degree-4 table
-//      (icnv_emission_table.inc, |error| < 5e-13 checked against 50-digit arithmetic, + < 3e-14 for keeping
-//      the cubic / quartic coefficients in single precision); z beyond the
+//      (icnv_emission_table.inc, |error| < 4.5e-13 checked against 50-digit arithmetic, + < 4.8e-13 for keeping
+//      the cubic / quartic coefficients to 20 mantissa bits, see the kernel); z beyond the
 //      table falls back to the nmath evaluation.
 //  (2) max_j(nu[j] + logPi[j,k]) uses the structure of .get_HMM's matrix (one diagonal value a,
 //      one off-diagonal value b, R/inferCNV_HMM.R:233-238): the winner is either "stay" (nu[k]+a)
-//      or the best other state (+b), found from the top three of nu+b, with which.max's
-//      first-index rule.
+//      or the best state (+b), with which.max's first-index rule.  The scores are kept minus i * a
+//      (a shift common to all states), so per gene nu'[k] = max(nu[k], best - cmove) + le[k], cmove = a - b.
 // Certificate: every arg-max (all states, all genes, and the final one) records the gap between
-// winner and runner-up.  Scores of the two arithmetics differ by at most n * (table error +
-// rounding) ~ 1e-8 for n <= 3000, so a sequence whose smallest gap exceeds tau = 1e-7 has the same
-// trace in both (tau is 2^-23 in the launcher).  Sequences below tau are appended to a list and recomputed by the exact kernel
-// above (list mode); their count is reported.
+// winner and runner-up; a sequence whose smallest gap exceeds tau = 2^-23 = 1.19e-7 has the same trace in both
+// arithmetics, the others are appended to a list and recomputed by the exact kernel above (list mode); their count is
+// reported.  Error budget, per gene and path, while every score is below 2^15 in magnitude (half an ulp <= 2^-38 = 3.6e-12;
+// checked at the end of the sequence): this pass rounds twice (best - cmove, + le) and its emission is off by < 9.3e-13
+// (table + shortened coefficients); the reference-order kernel rounds twice (nu + logPi, + le) and its emission is within
+// a few ulp of |le| <= 6, < 1e-14; cmove itself is rounded once (< 7.2e-15 for cmove < 64).  Together < 1.6e-11 per gene, so
+// the two arithmetics' scores of one path differ by < n * 1.6e-11, two paths' difference by twice that, and the rounded gap
+// e adds 3.6e-12: for n <= FAST_MAX_N = 3600 genes that is < 1.16e-7 < tau.  The longest sequence of the benchmark's layouts
+// (chromosome 1 at 20 000 genes, ~1 700 genes) stays below 5.5e-8.  Longer sequences go to the exact kernel.
 #include "icnv_emission_table.inc"
 
+constexpr int FAST_MAX_N = 3600;   // longest sequence the error budget above certifies
 constexpr int TG = 8;        // genes per staged tile
 constexpr int TS = TG + 1;   // padded row stride in doubles (bank-conflict-free column reads)
 constexpr int FAST_WARPS = 16;   // default warps per CTA (one CTA per SM: the replicated table below is shared by all of them);
@@ -373,8 +384,25 @@ __device__ __noinline__ double emission_far(double x, double mean, double sd) {
 }
 
 // acc += (v >= lim): a compare and a predicated add (the compiler's own form is compare, select 0 / 1, add)
-__device__ __forceinline__ void count_if_ge(int &acc, double v, double lim) {
-    asm("{ .reg .pred p; setp.ge.f64 p, %1, %2; @p add.s32 %0, %0, 1; }" : "+r"(acc) : "d"(v), "d"(lim));
+__device__ __forceinline__ void count_if_ge(int &acc, int v, int lim) {
+    asm("{ .reg .pred p; setp.ge.s32 p, %1, %2; @p add.s32 %0, %0, 1; }" : "+r"(acc) : "r"(v), "r"(lim));
+}
+
+// c3 rounded to 20 mantissa bits, as the high word of a double whose low word `lo` is already taken (c4's high word): of
+// the three high words around c3's own, the one whose pair lies nearest to c3 - within half a unit of the high word,
+// |error| <= 2^-21 |c3|
+__device__ __forceinline__ int c3_high_word(double c3, int lo) {
+    const int h = __double2hiint(c3);
+    int best = h;
+    double err = fabs(__hiloint2double(h, lo) - c3);
+    for (int d = -1; d <= 1; d += 2) {
+        const double e = fabs(__hiloint2double(h + d, lo) - c3);
+        if (e < err) {
+            err = e;
+            best = h + d;
+        }
+    }
+    return best;
 }
 
 // both 16-byte halves of interval `idx` from the lane's table replica (`tab_lane` -> its copy of interval 0): the address is
@@ -388,11 +416,14 @@ __device__ __forceinline__ void table_entry(const double2 *tab_lane, int idx, do
     asm volatile("ld.shared.v2.f64 {%0, %1}, [%2+%3];" : "=d"(c2f.x), "=d"(c2f.y) : "r"(addr), "n"(NTAB_BYTES));
 }
 
-template <int M, int NWARPS>
+template <int M, int NWARPS, bool SDCOL>
 __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitParams p) {
     extern __shared__ __align__(16) double sm[];
-    // emission table re-laid as [interval][replica] -> {c0, c1} and {c2, (float c3, float c4)}: two 16-byte loads
-    // per state (32 B instead of 40 B; c3, c4 only weigh u^3, u^4 with |u| <= 1/2: single precision costs < 3e-14).
+    // emission table re-laid as [interval][replica] -> {c0, c1} and {c2, c34}: two 16-byte loads per state (32 B instead
+    // of 40 B).  c34 holds c3 and c4 shortened to their high words (20 mantissa bits): read as a double it IS c3 (high word
+    // c3's, low word c4's high word, see c3_high_word), and c4 is its low word moved into a high word.  So the whole
+    // polynomial runs in FP64 without a conversion.  c3, c4 only weigh u^3, u^4 with |u| <= 1/2: the shortening costs
+    // <= 2^-21 * 7.9e-6 / 8 + 2^-20 * 5.0e-8 / 16 < 4.8e-13 (the table's largest |c3|, |c4|).
     // The lanes of a warp look up unrelated intervals, which on a single copy costs ~2.4 x the minimum number of
     // shared-memory wavefronts in bank conflicts - the table reads are this kernel's tightest resource.  With
     // TAB_REP = 8 copies interleaved at 16-byte granularity, lane l always reads bank group l & 7: every quarter
@@ -405,8 +436,8 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
     for (int e = threadIdx.x; e < ICNV_EMIS_N * TAB_REP; e += blockDim.x) {
         const int i = e / TAB_REP;
         tab01[e] = make_double2(p.table[i], p.table[ICNV_EMIS_N + i]);
-        const float c3 = (float)p.table[3 * ICNV_EMIS_N + i], c4 = (float)p.table[4 * ICNV_EMIS_N + i];
-        tab2f[e] = make_double2(p.table[2 * ICNV_EMIS_N + i], __hiloint2double(__float_as_int(c4), __float_as_int(c3)));
+        const int c4_hi = __double2hiint(p.table[4 * ICNV_EMIS_N + i]);
+        tab2f[e] = make_double2(p.table[2 * ICNV_EMIS_N + i], __hiloint2double(c3_high_word(p.table[3 * ICNV_EMIS_N + i], c4_hi), c4_hi));
     }
     __syncthreads();
     // this lane's replica of interval 0; the second halves (tab2f) follow at a constant distance
@@ -416,38 +447,42 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
     // backpointers: one 16-bit word per gene and lane - the best previous state (3 bits) and, per state, whether the
     // path into it comes from that best state (1) or stays (0)
     uint16_t *__restrict__ bp = reinterpret_cast<uint16_t *>(p.bp + warp_global * (int64_t)p.max_len * 32);
-    const double a = p.a_diag, b = p.b_off;
+    const double cmove = p.cmove;   // read from the parameter bank where it is used: no register held for it
     const double MAGIC = 6755399441055744.0;  // 1.5 * 2^52: (v + MAGIC) - MAGIC == rint(v), low word == (int)rint(v)
-    const int tau_hi = __double2hiint(p.tau);
     const unsigned long long pol = l2_evict_first_policy(p.evict_first == 1);
     const unsigned long long pol_ring = l2_evict_last_policy();
-    const double e_lim = (a - b) - p.tau;   // the launcher refuses the fast path unless a - b > 4 tau
+    // a state is "near the best" when its e = score - (best - cmove) reaches cmove - tau (> 0: the launcher refuses the fast
+    // path unless cmove > 8 tau).  Compared by high words: e >= cmove - tau implies hi(e) >= lim_hi, so the count can only
+    // come out too large - i.e. the check rejects a little more than the exact one would (a gap below tau + one unit of the
+    // high word, 2^-17 for cmove in [8, 16)), and never accepts what the exact one rejects
+    const int lim_hi = p.near_hi;   // __double2hiint(cmove - tau), from the launcher (a parameter-bank operand)
     int err = 0;
 
-    // second pass with at most 32 chromosomes: lane l holds the number of 32-sequence tiles of chromosomes 0 .. l (a warp scan
-    // of the list lengths), an item number below the total names (chromosome, tile) directly - no empty items are drawn
     const bool seq_compact = p.seq_mode && p.K <= 32;
-    long long seq_pre = 0, seq_total = 0;
-    if (seq_compact) {
-        long long t = lane < p.K ? ((long long)p.seq_counts[lane] + 31) / 32 : 0;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const long long u = __shfl_up_sync(0xffffffffu, t, d);
-            if (lane >= d) t += u;
-        }
-        seq_pre = t;
-        seq_total = __shfl_sync(0xffffffffu, t, 31);
-    }
     for (;;) {
         unsigned long long item = 0;
         if (lane == 0) item = atomicAdd(p.counter, 1ull);
+        // second pass with at most 32 chromosomes: lane l holds the number of 32-sequence tiles of chromosomes 0 .. l (a warp
+        // scan of the list lengths), an item number below the total names (chromosome, tile) directly - no empty items are
+        // drawn.  Formed per item: held across the gene loop, the two words would be spilled
+        unsigned seq_pre = 0, seq_total = 0;   // at most C + 32 tiles
+        if (seq_compact) {
+            unsigned t = lane < p.K ? (p.seq_counts[lane] + 31) / 32 : 0;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const unsigned u = __shfl_up_sync(0xffffffffu, t, d);
+                if (lane >= d) t += u;
+            }
+            seq_pre = t;
+            seq_total = __shfl_sync(0xffffffffu, t, 31);
+        }
         item = __shfl_sync(0xffffffffu, item, 0);
         if ((int64_t)item >= (seq_compact ? seq_total : p.n_items)) break;
         int ks = (int)(item / (unsigned long long)p.n_tiles);
         int64_t tile = (int64_t)(item % (unsigned long long)p.n_tiles);
         if (seq_compact) {
-            ks = __popc(__ballot_sync(0xffffffffu, seq_pre <= (long long)item));
-            const long long before = __shfl_sync(0xffffffffu, seq_pre, (ks + 31) & 31);   // lane ks - 1 (unused for ks = 0)
+            ks = __popc(__ballot_sync(0xffffffffu, seq_pre <= item));
+            const unsigned before = __shfl_sync(0xffffffffu, seq_pre, (ks + 31) & 31);   // lane ks - 1 (unused for ks = 0)
             tile = (int64_t)item - (ks > 0 ? before : 0);
         }
         const int cs = p.item_chr_start[ks];
@@ -467,11 +502,14 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
             if (active && n == 1) scol[cs] = 3;
             continue;
         }
-        const double sd = p.sd_col ? p.sd_col[cc] : p.sd;
-        const double scale = (double)ICNV_EMIS_INVW / sd;   // zs = 16 * |x - mean| / sd
-        double nms[MAXM];                                   // zs_k = |fma(x, scale, -mean_k * scale)|: one operation per state
+        const double sd = SDCOL ? p.sd_col[cc] : p.sd;
+        // zs_k = 16 * |x - mean_k| / sd = |fma(x, scale, -mean_k * scale)|: one operation per state.  With one sd for the
+        // launch, scale and the offsets are the launcher's (same operations, same bits) and stay in the parameter bank: held
+        // per lane they cost 12 registers, and under the 128-register cap the compiler would form them again every gene
+        const double scale = SDCOL ? (double)ICNV_EMIS_INVW / sd : p.emis_scale;
+        double nms[MAXM];
 #pragma unroll
-        for (int k = 0; k < M; ++k) nms[k] = -p.mean[k] * scale;
+        for (int k = 0; k < M; ++k) nms[k] = SDCOL ? -p.mean[k] * scale : p.emis_nms[k];
         const int g_lo = cs, g_hi = cs + n;
         const int b_first = g_lo / TG, b_last = (g_hi - 1) / TG;
 
@@ -512,7 +550,10 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
             __syncwarp();
             const double *row = tiles + buf * (32 * TS) + lane * TS;
             const int j0 = max(0, g_lo - blk * TG), j1 = min(TG, g_hi - blk * TG);
-#pragma unroll 1
+            // two genes per trip: the next gene's table lookups and polynomials are independent of this gene's recursion, so
+            // the compiler can issue them into its dependency gaps (3 % off the kernel at c3).  With per-lane offsets
+            // (SDCOL) the registers for that are not there: one gene per trip, spill-free
+#pragma unroll(SDCOL ? 1 : 2)
             for (int j = j0; j < j1; ++j) {
                 const int i = blk * TG + j - g_lo;
                 const double x = row[j];   // a non-finite x makes every zs NaN / Inf: it is caught on the rare path below
@@ -535,8 +576,8 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                         const double u = zs[k] - (m - MAGIC);
                         double2 c01, c2f;
                         table_entry(tab_lane, __double2loint(m), c01, c2f);
-                        const float hi = fmaf((float)u, __int_as_float(__double2hiint(c2f.y)), __int_as_float(__double2loint(c2f.y)));
-                        double v = fma(u, (double)hi, c2f.x);
+                        double v = fma(u, __hiloint2double(__double2loint(c2f.y), 0), c2f.y);   // c3 + u c4
+                        v = fma(u, v, c2f.x);
                         v = fma(u, v, c01.y);
                         le[k] = fma(u, v, c01.x);
                     }
@@ -550,8 +591,8 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                             const double u = zs[k] - (m - MAGIC);
                             double2 c01, c2f;
                             table_entry(tab_lane, __double2loint(m), c01, c2f);
-                            const float hi = fmaf((float)u, __int_as_float(__double2hiint(c2f.y)), __int_as_float(__double2loint(c2f.y)));
-                            v = fma(u, (double)hi, c2f.x);
+                            v = fma(u, __hiloint2double(__double2loint(c2f.y), 0), c2f.y);
+                            v = fma(u, v, c2f.x);
                             v = fma(u, v, c01.y);
                             v = fma(u, v, c01.x);
                         } else {
@@ -565,36 +606,46 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                     for (int k = 0; k < M; ++k) nu[k] = p.logdelta[k] + le[k];
                     continue;
                 }
-                // ---- T1 = max_k (nu[k] + b) and its first index: a compare / select chain carries the index along (strict
-                //      comparison = which.max's first-index rule; scores stay unperturbed, so the certificate's error budget
-                //      is the table error and rounding only) ----
-                double t[MAXM];
+                // ---- shifted frame: nu holds the scores minus i * a (a common shift: no arg-max sees it), so staying adds
+                //      nothing and coming from the best state costs cmove:  nu'[k] = max(nu[k], best - cmove) + le[k].
+                //      best = max_k nu[k] and its first index: a tournament of compare / select pairs carries the index along,
+                //      the lower-indexed side on the left (strict comparison = which.max's first-index rule).  M - 1
+                //      compares as in a chain, but ceil(log2 M) deep: this is the one step of the gene on the recursion's
+                //      dependency chain that has width ----
+                double bv[MAXM];
+                int bi[MAXM];
 #pragma unroll
-                for (int k = 0; k < M; ++k) t[k] = nu[k] + b;
-                double T1 = t[0];
-                int i1 = 0;
-#pragma unroll
-                for (int k = 1; k < M; ++k) {
-                    const bool gt = t[k] > T1;   // compare + select: fmax() is ~8 instructions in FP64
-                    T1 = gt ? t[k] : T1;
-                    i1 = gt ? k : i1;
+                for (int k = 0; k < M; ++k) {
+                    bv[k] = nu[k];
+                    bi[k] = k;
                 }
-                // ---- per state: stay (nu[k] + a) or come from the best state (T1).  With a > b the best
-                //      state always stays, so the runner-up is never a third state unless T1 - t[k] is
-                //      itself small - which the second check catches. --------------------------------------
+#pragma unroll
+                for (int s = 1; s < M; s *= 2) {
+#pragma unroll
+                    for (int k = 0; k + s < M; k += 2 * s) {
+                        const bool gt = bv[k + s] > bv[k];   // compare + select: fmax() is ~8 instructions in FP64
+                        bv[k] = gt ? bv[k + s] : bv[k];
+                        bi[k] = gt ? bi[k + s] : bi[k];
+                    }
+                }
+                const double best = bv[0];
+                const int i1 = bi[0];
+                const double T = best - cmove;   // "come from the best state"
+                // ---- per state: stay (nu[k]) or come from the best state (T).  The best state always stays (e = cmove),
+                //      so the runner-up is never a third state unless best - nu[k] is itself small - which the second
+                //      check catches. ----------------------------------------------------------------------------------
                 uint32_t moved = 0;   // bit k: the path into state k comes from the best state (sign bit of e, shifted in)
 #pragma unroll
                 for (int k = M - 1; k >= 0; --k) {
-                    const double d = nu[k] + a;
-                    const double e = d - T1;
+                    const double e = nu[k] - T;
                     const int he = __double2hiint(e);
                     const bool stay = he >= 0;
                     mg = min(mg, (unsigned)(he & 0x7fffffff));                      // |stay - from_best|
-                    // best vs every other state: T1 - t[k] = (a - b) - e up to three roundings of the scores, so the gap is
-                    // at least tau iff e <= a - b - tau.  The best state itself has e = a - b: exactly one state per gene may
-                    // exceed the bound - counted here, checked against the number of steps at the end of the sequence.
-                    count_if_ge(near_best, e, e_lim);
-                    nu[k] = (stay ? d : T1) + le[k];
+                    // best vs every other state: best - nu[k] = cmove - e up to two roundings, so the gap is at least tau
+                    // iff e <= cmove - tau.  The best state itself has e = cmove: exactly one state per gene may reach the
+                    // bound - counted here on the high word (see lim_hi), checked against the number of steps at the end.
+                    count_if_ge(near_best, he, lim_hi);
+                    nu[k] = (stay ? nu[k] : T) + le[k];
                     moved = __funnelshift_l((uint32_t)he, moved, 1);
                 }
                 bp_store(bp + (int64_t)i * 32 + lane, (uint16_t)(moved | ((uint32_t)i1 << 8)), pol_ring, p.evict_first >= 2);
@@ -621,9 +672,12 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
             const double gap = best - second;
             if (!(gap >= p.tau)) mg = 0;   // also catches NaN
             if (near_best != n - 1) mg = 0;   // some step had a second state within tau of the best one (or a NaN score)
+            // |score| < 2^15 keeps every rounding of the recursion below 2^-38 (error budget above); the best score rises by
+            // at most g(0) < 0.375 per gene, so a final best score above this bound means every earlier one was inside it
+            if (!(best - 0.375 * n > -32768.0 + cmove + 8.0) || n > FAST_MAX_N) mg = 0;
         }
         // uncertified sequences go to the exact kernel
-        if (active && (int)mg < tau_hi) {
+        if (active && (int)mg < __double2hiint(p.tau)) {
             unsigned pos = atomicAdd(p.list_out_count, 1u);
             if (pos < p.list_cap) p.list_out[pos] = make_int2(p.item_chr_id[ks], (int)c);
         }
@@ -1130,6 +1184,15 @@ int icnv_dev_scatter_group_states(const uint8_t *gs, int64_t G, int64_t C, const
     return ICNV_OK;
 }
 
+// the certified FP64 kernel for m states, fw warps per CTA (16, 20 or 24) and a per-column or launch-wide sd
+static void (*fast_kernel_for(int m, int fw, bool sd_col))(const VitParams) {
+    if (sd_col)
+        return (m == 6) ? (fw == 24 ? viterbi_fast_kernel<6, 24, true> : (fw == 20 ? viterbi_fast_kernel<6, 20, true> : viterbi_fast_kernel<6, 16, true>))
+                        : (fw == 24 ? viterbi_fast_kernel<3, 24, true> : (fw == 20 ? viterbi_fast_kernel<3, 20, true> : viterbi_fast_kernel<3, 16, true>));
+    return (m == 6) ? (fw == 24 ? viterbi_fast_kernel<6, 24, false> : (fw == 20 ? viterbi_fast_kernel<6, 20, false> : viterbi_fast_kernel<6, 16, false>))
+                    : (fw == 24 ? viterbi_fast_kernel<3, 24, false> : (fw == 20 ? viterbi_fast_kernel<3, 20, false> : viterbi_fast_kernel<3, 16, false>));
+}
+
 int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len, int K,
                          int m, const double *Pi, const double *delta, const double *mean, const double *sd,
                          int sd_per_col, uint8_t *states_u8, double *margins, int *err_flag, void *stream) {
@@ -1257,7 +1320,16 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
     p.a_diag = p.logPi[0];
     p.b_off = p.logPi[1];
     p.inv_sd = sd_per_col ? 0.0 : 1.0 / p.sd;
+    p.emis_scale = sd_per_col ? 0.0 : (double)ICNV_EMIS_INVW / p.sd;
+    for (int k = 0; k < MAXM; ++k) p.emis_nms[k] = (sd_per_col || k >= m) ? 0.0 : -p.mean[k] * p.emis_scale;
     p.tau = 1.1920928955078125e-07;  // 2^-23: power of two, so the high-word comparison in the kernel is exact
+    p.cmove = p.a_diag - p.b_off;
+    {
+        const double lim = p.cmove - p.tau;
+        int32_t hi;
+        std::memcpy(&hi, reinterpret_cast<const char *>(&lim) + 4, 4);
+        p.near_hi = hi;
+    }
     p.table = d_table;
     p.list_out = d_list;
     p.list_out_count = c.hmm_list_count;
@@ -1298,7 +1370,7 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
         ICNV_CHECK_LAUNCH("viterbi_fast32_kernel");
         // second pass: the sequences the single-precision margins could not certify, 32 of one chromosome per warp, in the FP64
         // arithmetic with its own (all-decisions) certificate; what that rejects goes on to the reference-order kernel
-        void (*fkern64)(const VitParams) = (m == 6) ? viterbi_fast_kernel<6, 16> : viterbi_fast_kernel<3, 16>;
+        void (*fkern64)(const VitParams) = fast_kernel_for(m, FAST_WARPS, sd_per_col != 0);
         const size_t smem64 = sizeof(double) * (4 * (ICNV_EMIS_N + 1) * TAB_REP + (size_t)FAST_WARPS * 2 * 32 * TS);
         ICNV_CUDA(cudaFuncSetAttribute(fkern64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem64));
         p.seq_mode = 1;
@@ -1318,9 +1390,7 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
     int fw = FAST_WARPS;
     if (c.opt_vfast_warps) fw = c.opt_vfast_warps;   // read once in icnv_init
     if (fw != 16 && fw != 20 && fw != 24) fw = FAST_WARPS;
-    void (*fkern)(const VitParams) =
-        (m == 6) ? (fw == 24 ? viterbi_fast_kernel<6, 24> : (fw == 20 ? viterbi_fast_kernel<6, 20> : viterbi_fast_kernel<6, 16>))
-                 : (fw == 24 ? viterbi_fast_kernel<3, 24> : (fw == 20 ? viterbi_fast_kernel<3, 20> : viterbi_fast_kernel<3, 16>));
+    void (*fkern)(const VitParams) = fast_kernel_for(m, fw, sd_per_col != 0);
     const size_t smem = sizeof(double) * (4 * (ICNV_EMIS_N + 1) * TAB_REP + (size_t)fw * 2 * 32 * TS);
     p.means_monotone = 1;
     for (int k = 1; k + 1 < m; ++k)
