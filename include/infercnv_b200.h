@@ -245,6 +245,18 @@ ICNV_API int icnv_pairwise_dist_f64(const double *X, int64_t G, int64_t C, const
  * closure passes its argument through without transposing it back. */
 ICNV_API int icnv_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t G, double *out);
 
+/* hclust(d, method) - fastcluster::hclust, which infercnv imports - on R's "dist" vector d of n observations (the layout
+ * above).  Nearest-neighbour chain with Lance-Williams updates on an n x n FP64 matrix on the device (n^2 * 8 bytes; the
+ * host vector goes in slab by slab).  method, coded as fastcluster orders them: 0 single, 1 complete, 2 average,
+ * 3 mcquitty, 4 ward.D, 7 ward.D2 (ward.D on the squared input, heights rooted).  5 centroid / 6 median and n > 65536:
+ * ICNV_E_UNSUPPORTED; NaN / Inf in d: ICNV_E_NONFINITE; n < 2 or another code: ICNV_E_BAD_ARG; no room: ICNV_E_NOMEM.
+ * Output in R's convention: merge (n - 1) x 2 column-major (singleton -(i + 1), cluster of step s +s, the smaller node
+ * first), height (n - 1, non-decreasing), order (n, 1-based).  Tie rules: see icnv_hclust.cu. */
+ICNV_API int icnv_hclust_f64(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order);
+/* R's order from merge: hcass2's traversal (start from the last merge, expand the first column before the second).
+ * Host only, no GPU. */
+ICNV_API int icnv_hclust_order(const int32_t *merge, int64_t n, int32_t *order);
+
 /* Combine per-cell (sum, sd) pairs - e.g. all-gathered from several GPUs - into mu / sigma over all values
  * of those cells, in list order (what icnv_mean_sd_f64 does internally). */
 ICNV_API void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, int64_t G, double *mu,
@@ -410,6 +422,10 @@ ICNV_API int icnv_dev_median_filter_f64(const double *X, double *Y, int64_t G, i
 ICNV_API int icnv_dev_pairwise_dist_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
                                         double *out, void *stream);
 ICNV_API int icnv_dev_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t ldx, int64_t G, double *out, void *stream);
+/* icnv_hclust_f64 on a device "dist" vector: merge / height (device) as above, no order (icnv_hclust_order on the host
+ * copy of merge).  Synchronises the stream once, after filling the matrix, to report non-finite input; the linkage itself
+ * is enqueued on `stream`. */
+ICNV_API int icnv_dev_hclust_f64(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream);
 /* Region calling on device-resident states (uint8, column stride lds >= G).
  * icnv_dev_state_counts_u8: counts[(k*G + g)*8 + slot] = number of cells of group k (d_cells[h_grp_off[k] ..
  * h_grp_off[k+1]), device) whose state at gene g falls in `slot` (0: unassigned, v+1: state v); integer counts, so

@@ -307,6 +307,48 @@ def pairwise_dist_rows(x, out=None):
     return out
 
 
+# hclust() methods with an exact nearest-neighbour chain, coded as fastcluster orders them (centroid 5 and median 6 are not
+# reducible and have no GPU path)
+HCLUST_METHODS = {"single": 0, "complete": 1, "average": 2, "mcquitty": 3, "ward.D": 4, "ward.D2": 7}
+
+
+def hclust_method_code(method) -> int:
+    if isinstance(method, str):
+        if method not in HCLUST_METHODS:
+            raise ValueError(f"hclust method {method!r}: one of {sorted(HCLUST_METHODS)}")
+        return HCLUST_METHODS[method]
+    return int(method)
+
+
+def _dist_size(n_d: int) -> int:
+    n = int(round((1 + np.sqrt(1 + 8 * n_d)) / 2))
+    if n * (n - 1) // 2 != n_d:
+        raise ValueError(f"{n_d} entries are not a \"dist\" vector (n (n - 1) / 2 for some n)")
+    return n
+
+
+def hclust(d, method="ward.D2"):
+    """fastcluster::hclust(d, method) on R's "dist" vector d (strict lower triangle by columns, e.g. pairwise_dist's
+    output): returns (merge, height, order) in R's convention - merge (n - 1) x 2 int32 (singleton -(i + 1), cluster of
+    step s +s), height (n - 1), order (n, 1-based).  Methods: HCLUST_METHODS (or their codes)."""
+    d = np.ascontiguousarray(d, dtype=np.float64).ravel()
+    n = _dist_size(d.size)
+    merge = np.empty((max(n - 1, 0), 2), dtype=np.int32, order="F")
+    height = np.empty(max(n - 1, 0), dtype=np.float64)
+    order = np.empty(n, dtype=np.int32)
+    _lib.check(_lib.load().icnv_hclust_f64(_p(d), n, hclust_method_code(method), _p(merge), _p(height), _p(order)))
+    return merge, height, order
+
+
+def hclust_order(merge) -> np.ndarray:
+    """R's `order` from a merge matrix ((n - 1) x 2): hcass2's traversal, on the host (icnv_hclust_order)."""
+    m = np.asfortranarray(merge, dtype=np.int32)
+    n = m.shape[0] + 1
+    order = np.empty(n, dtype=np.int32)
+    _lib.check(_lib.load().icnv_hclust_order(_p(m), n, _p(order)))
+    return order
+
+
 # ---- CNV region calling on the state matrix (R/inferCNV_HMM.R:706-1087) ---------------------------------------
 
 def _u8(a) -> np.ndarray:

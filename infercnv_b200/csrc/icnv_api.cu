@@ -1783,3 +1783,53 @@ void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, i
 }
 
 }  // extern "C"
+
+// ---- hclust (kernels and bodies in icnv_hclust.cu) ---------------------------------------------------------------------
+// Weak references: a library built without icnv_hclust.cu - the host emulation of the other kernels' source - still loads
+// and exports every entry point of the header; there the linkage entry points report ICNV_E_UNSUPPORTED.
+namespace icnv {
+int hclust_host(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order) __attribute__((weak));
+int hclust_dev(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream) __attribute__((weak));
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_hclust_f64(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order) {
+    if (!icnv::hclust_host) return set_error(ICNV_E_UNSUPPORTED, "icnv_hclust_f64: this build has no linkage kernel");
+    return icnv::hclust_host(d, n, method, merge, height, order);
+}
+
+int icnv_dev_hclust_f64(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream) {
+    if (!icnv::hclust_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_hclust_f64: this build has no linkage kernel");
+    return icnv::hclust_dev(d_dist, n, method, merge, height, stream);
+}
+
+// R's order: hcass2's traversal - start from the last merge, expand the first column before the second.
+int icnv_hclust_order(const int32_t *merge, int64_t n, int32_t *order) {
+    if (!merge || !order || n < 1) return set_error(ICNV_E_BAD_ARG, "icnv_hclust_order: bad argument");
+    if (n == 1) {
+        order[0] = 1;
+        return ICNV_OK;
+    }
+    const int64_t nm = n - 1;
+    std::vector<int32_t> stack;
+    stack.reserve((size_t)n);
+    stack.push_back((int32_t)nm);   // 1-based merge number
+    int64_t out = 0;
+    while (!stack.empty()) {
+        const int32_t v = stack.back();
+        stack.pop_back();
+        if (v < 0) {
+            if (out >= n || -v > n) return set_error(ICNV_E_BAD_ARG, "icnv_hclust_order: merge is not a tree");
+            order[out++] = -v;
+            continue;
+        }
+        if (v < 1 || v > nm) return set_error(ICNV_E_BAD_ARG, "icnv_hclust_order: merge is not a tree");
+        stack.push_back(merge[nm + v - 1]);
+        stack.push_back(merge[v - 1]);
+    }
+    if (out != n) return set_error(ICNV_E_BAD_ARG, "icnv_hclust_order: merge is not a tree");
+    return ICNV_OK;
+}
+
+}  // extern "C"

@@ -394,6 +394,20 @@ class Engine:
                                                        n, out.data_ptr(), _stream_ptr()))
         return out
 
+    def hclust(self, D, n, method="ward.D2"):
+        """hclust() on the device "dist" vector D of n observations (what pairwise_dist returns), fastcluster's methods
+        (api.HCLUST_METHODS): (merge, height, order) as numpy arrays in R's convention.  Only merge comes back to the
+        host before `order` is computed from it; height follows with it."""
+        from .api import hclust_method_code, hclust_order
+        if D.dtype != torch.float64 or not D.is_contiguous() or D.numel() != n * (n - 1) // 2:
+            raise ValueError("D must be a contiguous float64 device vector of n (n - 1) / 2 entries")
+        merge = torch.empty((2, max(n - 1, 0)), dtype=torch.int32, device=self.tdev)   # column-major (n - 1) x 2
+        height = torch.empty(max(n - 1, 0), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_hclust_f64(D.data_ptr(), n, hclust_method_code(method), merge.data_ptr(),
+                                                height.data_ptr(), _stream_ptr()))
+        m = merge.cpu().numpy().T
+        return m, height.cpu().numpy(), hclust_order(m)
+
     def mean_sd(self, X, groups_local):
         """mu / sigma over all values of the listed cells across ALL ranks (.i3HMM_get_sd_trend_by_num_cells_fit,
         R/inferCNV_i3HMM.R:17-30).  groups_local: per group, this rank's LOCAL columns (the planner's slices).

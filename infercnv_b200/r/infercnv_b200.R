@@ -457,6 +457,31 @@ b200_parallelDist <- function(x, method = "euclidean", diag = FALSE, upper = FAL
     orig(x, method = method, diag = diag, upper = upper, threads = threads, ...)
 }
 
+## fastcluster::hclust as infercnv calls it on every parallelDist() result - hclust(d, method = hclust_method), default
+## "ward.D2" (R/inferCNV_ops.R:262; R/inferCNV_tumor_subclusters.R:191,411,474,498,582,609; R/inferCNV_ops.R:1930,3242;
+## R/inferCNV_heatmap.R:719,755,1062,1079).  Same signature as fastcluster::hclust(d, method = "complete", members = NULL)
+## and the same "hclust" object.  The six reducible methods run as a nearest-neighbour chain on the GPU; anything else - not
+## a "dist", non-NULL members, centroid / median / the alias "ward", fewer than 2 or more than 65 536 observations, NA in
+## d, or a library error - goes to the original.
+b200_hclust <- function(d, method = "complete", members = NULL) {
+    orig <- .icnv_env$orig_hclust
+    codes <- c(single = 0L, complete = 1L, average = 2L, mcquitty = 3L, ward.D = 4L, ward.D2 = 7L)
+    n <- if (inherits(d, "dist")) attr(d, "Size") else NA
+    ok <- .icnv_enabled() && inherits(d, "dist") && is.null(members) && is.character(method) && length(method) == 1 &&
+        method %in% names(codes) && !is.null(n) && !is.na(n) && n >= 2 && n <= 65536 && !anyNA(d)
+    if (ok) {
+        code <- codes[[method]]
+        res <- .icnv_try(.Call("icnvR_hclust", d, code), "hclust")
+        if (!is.null(res)) {
+            return(structure(list(merge = res[[1]], height = res[[2]], order = res[[3]], labels = attr(d, "Labels"),
+                                  method = method, call = match.call(), dist.method = attr(d, "method")),
+                             class = "hclust"))
+        }
+    }
+    if (is.null(orig)) orig <- fastcluster::hclust
+    orig(d, method = method, members = members)
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -476,6 +501,13 @@ infercnvb200_install <- function() {
         assign("parallelDist", b200_parallelDist, envir = imp)
         lockBinding("parallelDist", imp)
     }
+    ## hclust is an import too (NAMESPACE: importFrom(fastcluster, hclust))
+    if (exists("hclust", envir = imp, inherits = FALSE)) {
+        .icnv_env$orig_hclust <- get("hclust", envir = imp)
+        unlockBinding("hclust", imp)
+        assign("hclust", b200_hclust, envir = imp)
+        lockBinding("hclust", imp)
+    }
     invisible(TRUE)
 }
 
@@ -486,6 +518,11 @@ infercnvb200_uninstall <- function() {
         unlockBinding("parallelDist", imp)
         assign("parallelDist", .icnv_env$orig_parallelDist, envir = imp)
         lockBinding("parallelDist", imp)
+    }
+    if (!is.null(.icnv_env$orig_hclust)) {
+        unlockBinding("hclust", imp)
+        assign("hclust", .icnv_env$orig_hclust, envir = imp)
+        lockBinding("hclust", imp)
     }
     invisible(TRUE)
 }

@@ -11,6 +11,7 @@
  */
 #include <R.h>
 #include <Rinternals.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
 
@@ -235,6 +236,26 @@ SEXP icnvR_pairwise_dist(SEXP x) {
     return ans;
 }
 
+/* hclust(d, method) (fastcluster::hclust, an import of infercnv) on a "dist" vector d: method_code as in
+ * icnv_hclust_f64 (0 single, 1 complete, 2 average, 3 mcquitty, 4 ward.D, 7 ward.D2).  Returns list(merge (n-1) x 2
+ * INTSXP, height REALSXP, order INTSXP); the R closure adds labels / method / call / dist.method and the class. */
+SEXP icnvR_hclust(SEXP d, SEXP method_code) {
+    R_xlen_t len = Rf_xlength(d);
+    int64_t n = (int64_t)((1.0 + sqrt(1.0 + 8.0 * (double)len)) / 2.0 + 0.5);
+    if (n * (n - 1) / 2 != (int64_t)len || n < 2) Rf_error("infercnv_b200: not a \"dist\" vector of at least 2 observations");
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 3));
+    SEXP merge = Rf_allocMatrix(INTSXP, (int)(n - 1), 2);
+    SET_VECTOR_ELT(ans, 0, merge);
+    SEXP height = Rf_allocVector(REALSXP, (R_xlen_t)(n - 1));
+    SET_VECTOR_ELT(ans, 1, height);
+    SEXP order = Rf_allocVector(INTSXP, (R_xlen_t)n);
+    SET_VECTOR_ELT(ans, 2, order);
+    int rc = icnv_hclust_f64(REAL(d), n, Rf_asInteger(method_code), INTEGER(merge), REAL(height), INTEGER(order));
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* normalize_counts_by_seq_depth (ops.R:3064-3111); normalize_factor NA -> median of colSums */
 SEXP icnvR_normalize(SEXP expr, SEXP normalize_factor) {
     SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
@@ -412,7 +433,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_viterbi_per_chr", (DL_FUNC)&icnvR_viterbi_per_chr, 9}, {"icnvR_scale", (DL_FUNC)&icnvR_scale, 1},
     {"icnvR_clear_noise_threshold", (DL_FUNC)&icnvR_clear_noise_threshold, 4},
     {"icnvR_smooth_hmm", (DL_FUNC)&icnvR_smooth_hmm, 11},   {"icnvR_init_devices", (DL_FUNC)&icnvR_init_devices, 1},
-    {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1},
+    {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1}, {"icnvR_hclust", (DL_FUNC)&icnvR_hclust, 2},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -17,6 +17,7 @@ SEXP Rf_getAttrib(SEXP, SEXP);
 int *INTEGER(SEXP);
 double *REAL(SEXP);
 int Rf_length(SEXP);
+R_xlen_t Rf_xlength(SEXP);
 SEXP VECTOR_ELT(SEXP, long);
 SEXP SET_VECTOR_ELT(SEXP, long, SEXP);
 SEXP Rf_allocMatrix(unsigned, int, int);

@@ -658,3 +658,14 @@ def parallelDist(x, method: str = "euclidean", threads=None) -> np.ndarray:
     if x.ndim != 2:
         raise ValueError("x must be a matrix (observations x variables)")
     return api.pairwise_dist_rows(x)
+
+
+def hclust(d, method: str = "complete", members=None) -> dict:
+    """`hclust(d, method)` as infercnv calls it (fastcluster::hclust, imported by the reference; R/inferCNV_ops.R:262 passes
+    "ward.D2" by default) on a "dist" vector such as parallelDist()'s.  Returns a dict shaped like R's "hclust" object:
+    merge ((n - 1) x 2), height, order (1-based), labels, method, dist.method.  centroid / median and `members` are not
+    on the GPU."""
+    if members is not None:
+        raise NotImplementedError("hclust(members=...) is not on the GPU path")
+    merge, height, order = api.hclust(d, method)
+    return {"merge": merge, "height": height, "order": order, "labels": None, "method": method, "dist.method": "euclidean"}
