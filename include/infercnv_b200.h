@@ -245,6 +245,25 @@ ICNV_API int icnv_pairwise_dist_f64(const double *X, int64_t G, int64_t C, const
  * closure passes its argument through without transposing it back. */
 ICNV_API int icnv_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t G, double *out);
 
+/* RANN::nn2(data, k = k) with the query set = the data set - the kNN graph of .leiden_simple_snn,
+ * R/inferCNV_tumor_subclusters.R:725-741 (NAMESPACE: importFrom(RANN, nn2)): for each of the n cells its k nearest cells
+ * under the Euclidean distance over the genes, itself included.  Exact (no approximation, no n x n buffer: device memory is
+ * the input plus O(n k)).  idx / dist: n x k column-major, as R's nn.idx / nn.dists; idx holds 0-based list positions (the
+ * R shim adds 1).  Row i is ordered by ascending squared distance, then ascending position - a total order, so the result
+ * does not depend on the launch geometry, and cell i comes first in its row unless a duplicate of it has a lower position.
+ * ANN orders ties by its tree traversal, so among equally near cells the choice can differ from RANN's; only ties that
+ * straddle the k-th place change the neighbour set.  Distances are the square roots of the same sums as
+ * icnv_pairwise_dist_f64 (difference form, genes in order, one fused multiply-add each): every dist[i, j] has the bits of
+ * that pair's "dist" entry.  k < 1 or k > n: ICNV_E_BAD_ARG; k > ICNV_KNN_MAX_K: ICNV_E_UNSUPPORTED; NaN / Inf in a listed
+ * cell: ICNV_E_NONFINITE; n = 0: nothing is written; G = 0: every distance is 0, row i is 0 .. k-1.
+ * This entry takes the matrix as nn2() receives it: observations x variables, cell a / gene g at x[a + n g]. */
+#define ICNV_KNN_MAX_K 64
+ICNV_API int icnv_knn_rows_f64(const double *x, int64_t n, int64_t G, int k, int32_t *idx, double *dist);
+/* The same from the genes x cells matrix X (G x C, column-major) and a list of n 0-based columns (NULL: all C columns in
+ * order, n is then ignored), as icnv_pairwise_dist_f64 takes them. */
+ICNV_API int icnv_knn_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int k, int32_t *idx,
+                          double *dist);
+
 /* hclust(d, method) - fastcluster::hclust, which infercnv imports - on R's "dist" vector d of n observations (the layout
  * above).  Nearest-neighbour chain with Lance-Williams updates on an n x n FP64 matrix on the device (n^2 * 8 bytes; the
  * host vector goes in slab by slab).  method, coded as fastcluster orders them: 0 single, 1 complete, 2 average,
@@ -422,6 +441,11 @@ ICNV_API int icnv_dev_median_filter_f64(const double *X, double *Y, int64_t G, i
 ICNV_API int icnv_dev_pairwise_dist_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
                                         double *out, void *stream);
 ICNV_API int icnv_dev_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t ldx, int64_t G, double *out, void *stream);
+/* icnv_knn_f64 on device pointers: columns X + ldx * (d_cells ? d_cells[a] : a), a < n (a gene range - one chromosome - is
+ * X offset by its first gene, ldx unchanged); idx / dist: n x k column-major (device).  Both kernels are enqueued on
+ * `stream`, which is then synchronised once to report non-finite input. */
+ICNV_API int icnv_dev_knn_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int k,
+                              int32_t *idx, double *dist, void *stream);
 /* icnv_hclust_f64 on a device "dist" vector: merge / height (device) as above, no order (icnv_hclust_order on the host
  * copy of merge).  Synchronises the stream once, after filling the matrix, to report non-finite input; the linkage itself
  * is enqueued on `stream`. */

@@ -53,6 +53,9 @@ SIGNATURES = {
     "icnv_dev_pairwise_dist_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, _P, _P]),
     "icnv_pairwise_dist_rows_f64": (c_int, [_P, c_i64, c_i64, _P]),
     "icnv_dev_pairwise_dist_rows_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, _P]),
+    "icnv_knn_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, _P, _P]),
+    "icnv_knn_rows_f64": (c_int, [_P, c_i64, c_i64, c_int, _P, _P]),
+    "icnv_dev_knn_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, _P, _P, _P]),
     "icnv_hclust_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
     "icnv_dev_hclust_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
     "icnv_hclust_order": (c_int, [_P, c_i64, _P]),

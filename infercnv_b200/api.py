@@ -307,6 +307,39 @@ def pairwise_dist_rows(x, out=None):
     return out
 
 
+KNN_MAX_K = 64   # ICNV_KNN_MAX_K
+
+
+def _knn_out(n: int, k: int):
+    shape = (n, max(int(k), 0)) if n > 0 else (0, 0)
+    return np.empty(shape, dtype=np.int32, order="F"), np.empty(shape, dtype=np.float64, order="F")
+
+
+def knn(X, k, cells=None):
+    """The k nearest of the listed cells (default: all columns of the genes x cells matrix X) for each of them, itself
+    included - RANN::nn2(t(X[, cells]), k = k) exactly: (idx, dist), each (n, k), idx 0-based list positions.  Rows are
+    ordered by squared distance, then position (icnv_knn_f64); distances have the bits of pairwise_dist's."""
+    X = _f64(X)
+    G, C = X.shape
+    idx = None if cells is None else _i32(cells)
+    n = C if idx is None else len(idx)
+    nn_idx, nn_dist = _knn_out(n, k)
+    _lib.check(_lib.load().icnv_knn_f64(_p(X), G, C, _p(idx) if idx is not None else None, n, int(k), _p(nn_idx),
+                                        _p(nn_dist)))
+    return nn_idx, nn_dist
+
+
+def knn_rows(x, k):
+    """knn() on x = observations x variables, the matrix nn2() receives (t(expr.data[, cells])): icnv_knn_rows_f64."""
+    x = np.asfortranarray(np.asarray(x, dtype=np.float64))
+    if x.ndim != 2:
+        raise ValueError("x must be a matrix (observations x variables)")
+    n, G = x.shape
+    nn_idx, nn_dist = _knn_out(n, k)
+    _lib.check(_lib.load().icnv_knn_rows_f64(_p(x), n, G, int(k), _p(nn_idx), _p(nn_dist)))
+    return nn_idx, nn_dist
+
+
 # hclust() methods with an exact nearest-neighbour chain, coded as fastcluster orders them (centroid 5 and median 6 are not
 # reducible and have no GPU path)
 HCLUST_METHODS = {"single": 0, "complete": 1, "average": 2, "mcquitty": 3, "ward.D": 4, "ward.D2": 7}

@@ -62,6 +62,12 @@ extern "C" ICNV_API void icnv_combine_cell_stats(const double *sums, const doubl
                                                 double *sigma);
 
 namespace icnv {
+// K12 in either layout (icnv_dist.cu)
+int knn_launch(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int k, int32_t *idx, double *dist,
+               int rows, void *stream, const char *who);
+}  // namespace icnv
+
+namespace icnv {
 
 static thread_local char g_err[512] = "";
 
@@ -1764,6 +1770,42 @@ int icnv_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t G, double *o
     ICNV_CUDA(cudaMemcpyAsync(out, d_out, sizeof(double) * n_out, cudaMemcpyDeviceToHost, st));
     ICNV_CUDA(cudaStreamSynchronize(st));
     return ICNV_OK;
+}
+
+// k nearest neighbours: the input goes up whole (it is all K12 holds besides O(n k)), the n x k results come back
+static int knn_host(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int k, int32_t *idx, double *dist,
+                    int rows, const char *who) {
+    ICNV_HOST_PROLOGUE();
+    if (!X || G < 0 || n < 0 || (!rows && C < 0) || (n > 0 && (!idx || !dist))) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    for (int64_t i = 0; cells && i < n; ++i)
+        if (cells[i] < 0 || cells[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index out of range", who);
+    if (n == 0) return ICNV_OK;
+    if (k < 1 || k > n) return set_error(ICNV_E_BAD_ARG, "%s: k = %d for %lld cells (1 <= k <= n)", who, k, (long long)n);
+    if (k > ICNV_KNN_MAX_K) return set_error(ICNV_E_UNSUPPORTED, "%s: k = %d (limit %d)", who, k, ICNV_KNN_MAX_K);
+    const size_t nk = (size_t)n * (size_t)k;
+    double *d_dist = (double *)scratch(SLOT_OUT, (sizeof(double) + sizeof(int32_t)) * nk);
+    int32_t *d_idx = (int32_t *)(d_dist + nk);
+    int32_t *d_cells = cells ? (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * (size_t)n) : nullptr;
+    double *dX = nullptr;
+    int rc;
+    if (!d_dist || (cells && !d_cells)) return ICNV_E_NOMEM;
+    if (G > 0 && (rc = upload_matrix(X, G * (rows ? n : C), &dX, SLOT_IN, st))) return rc;
+    if (G == 0) dX = d_dist;   // never read
+    if (cells) ICNV_CUDA(cudaMemcpyAsync(d_cells, cells, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    if ((rc = knn_launch(dX, G, rows ? n : G, d_cells, n, k, d_idx, d_dist, rows, st, who))) return rc;
+    ICNV_CUDA(cudaMemcpyAsync(idx, d_idx, sizeof(int32_t) * nk, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaMemcpyAsync(dist, d_dist, sizeof(double) * nk, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return ICNV_OK;
+}
+
+int icnv_knn_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int k, int32_t *idx, double *dist) {
+    if (!cells) n = C;
+    return knn_host(X, G, C, cells, n, k, idx, dist, 0, "icnv_knn_f64");
+}
+
+int icnv_knn_rows_f64(const double *x, int64_t n, int64_t G, int k, int32_t *idx, double *dist) {
+    return knn_host(x, G, n, nullptr, n, k, idx, dist, 1, "icnv_knn_rows_f64");
 }
 
 /* mu, sigma (n-1) over all values of n cells from the cells' own (sum, sd): sum of squares about mu of a cell =

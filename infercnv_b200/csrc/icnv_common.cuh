@@ -52,6 +52,7 @@ enum ScratchSlot {
     SLOT_MF_PRE,                      // median filter: range of the matrix and the value sample of its pre-pass
     SLOT_TABLE32,                     // single-precision emission table
     SLOT_SEQ,                         // per-chromosome lists of the sequences for the FP64 second pass
+    SLOT_KNN,                         // k nearest neighbours: per-split partial lists and the non-finite flag
     SLOT_COUNT
 };
 

@@ -394,6 +394,23 @@ class Engine:
                                                        n, out.data_ptr(), _stream_ptr()))
         return out
 
+    def knn(self, X, k, cells=None):
+        """The k nearest of the listed local cells (rows of X; default all) for each of them, on the device - the nn2() of
+        .leiden_simple_snn (R/inferCNV_tumor_subclusters.R:725-741).  X is a (C, G) float64 tensor with contiguous genes,
+        or a gene-range view of one (X[:, a:b], one chromosome): the view's stride is the column stride.  Returns device
+        tensors (idx int32, dist float64), each (n, k) with 0-based list positions, as api.knn."""
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        G = X.shape[1]
+        idx = None if cells is None else torch.as_tensor(np.asarray(cells, dtype=np.int32), device=self.tdev)
+        n = X.shape[0] if idx is None else int(idx.numel())
+        kk = max(int(k), 0) if n > 0 else 0
+        nn_idx = torch.empty((kk, n), dtype=torch.int32, device=self.tdev)    # column-major n x k
+        nn_dist = torch.empty((kk, n), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_knn_f64(X.data_ptr(), G, max(X.stride(0), G), idx.data_ptr() if idx is not None else None,
+                                             n, int(k), nn_idx.data_ptr(), nn_dist.data_ptr(), _stream_ptr()))
+        return nn_idx.T, nn_dist.T
+
     def hclust(self, D, n, method="ward.D2"):
         """hclust() on the device "dist" vector D of n observations (what pairwise_dist returns), fastcluster's methods
         (api.HCLUST_METHODS): (merge, height, order) as numpy arrays in R's convention.  Only merge comes back to the

@@ -482,6 +482,27 @@ b200_hclust <- function(d, method = "complete", members = NULL) {
     orig(d, method = method, members = members)
 }
 
+## RANN::nn2 as .leiden_simple_snn calls it - nn2(t(expr_data), k = k_nn)$nn.idx (R/inferCNV_tumor_subclusters.R:725-741),
+## the kNN graph of the default per-chromosome Leiden subclustering.  Same signature as RANN::nn2(data, query = data,
+## k = min(10, nrow(data)), treetype = c("kd", "bd"), searchtype = c("standard", "priority", "radius"), radius = 0, eps = 0)
+## and the same list(nn.idx, nn.dists).  The exact search runs on the GPU when query is the data itself, data is a double
+## matrix without NA, searchtype is not "radius", eps is 0 and 1 <= k <= min(nrow(data), 64); anything else, or a library
+## error, goes to the original.  Among equally near cells the GPU takes the lowest row (ANN: its tree traversal).
+b200_nn2 <- function(data, query = data, k = min(10, nrow(data)), treetype = c("kd", "bd"),
+                     searchtype = c("standard", "priority", "radius"), radius = 0, eps = 0) {
+    orig <- .icnv_env$orig_nn2
+    st <- tryCatch(match.arg(searchtype), error = function(e) NA_character_)
+    ok <- .icnv_enabled() && (missing(query) || identical(query, data)) && is.matrix(data) && is.double(data) &&
+        !anyNA(data) && !is.na(st) && st != "radius" && is.numeric(eps) && length(eps) == 1 && isTRUE(eps == 0) &&
+        is.numeric(k) && length(k) == 1 && !is.na(k) && k == round(k) && k >= 1 && k <= min(nrow(data), 64)
+    if (ok) {
+        res <- .icnv_try(.Call("icnvR_knn", data, as.integer(k)), "nn2")
+        if (!is.null(res)) return(list(nn.idx = res[[1]], nn.dists = res[[2]]))
+    }
+    if (is.null(orig)) orig <- RANN::nn2
+    orig(data, query = query, k = k, treetype = treetype, searchtype = searchtype, radius = radius, eps = eps)
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -508,6 +529,13 @@ infercnvb200_install <- function() {
         assign("hclust", b200_hclust, envir = imp)
         lockBinding("hclust", imp)
     }
+    ## and nn2 (NAMESPACE: importFrom(RANN, nn2))
+    if (exists("nn2", envir = imp, inherits = FALSE)) {
+        .icnv_env$orig_nn2 <- get("nn2", envir = imp)
+        unlockBinding("nn2", imp)
+        assign("nn2", b200_nn2, envir = imp)
+        lockBinding("nn2", imp)
+    }
     invisible(TRUE)
 }
 
@@ -523,6 +551,11 @@ infercnvb200_uninstall <- function() {
         unlockBinding("hclust", imp)
         assign("hclust", .icnv_env$orig_hclust, envir = imp)
         lockBinding("hclust", imp)
+    }
+    if (!is.null(.icnv_env$orig_nn2)) {
+        unlockBinding("nn2", imp)
+        assign("nn2", .icnv_env$orig_nn2, envir = imp)
+        lockBinding("nn2", imp)
     }
     invisible(TRUE)
 }

@@ -256,6 +256,29 @@ SEXP icnvR_hclust(SEXP d, SEXP method_code) {
     return ans;
 }
 
+/* nn2(data, k = k) (RANN::nn2, an import of infercnv) with the query set = the data set, data = observations x variables
+ * (.leiden_simple_snn, R/inferCNV_tumor_subclusters.R:725-741).  Returns list(nn.idx n x k INTSXP, 1-based, nn.dists n x k
+ * REALSXP); the R closure names the fields. */
+SEXP icnvR_knn(SEXP x, SEXP k_) {
+    SEXP dim = Rf_getAttrib(x, R_DimSymbol);
+    int64_t n = INTEGER(dim)[0], G = INTEGER(dim)[1];
+    int k = Rf_asInteger(k_);
+    if (k < 1 || (int64_t)k > n) Rf_error("infercnv_b200: nn2() needs 1 <= k <= nrow(data)");
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 2));
+    SEXP idx = Rf_allocMatrix(INTSXP, (int)n, k);
+    SET_VECTOR_ELT(ans, 0, idx);
+    SEXP dist = Rf_allocMatrix(REALSXP, (int)n, k);
+    SET_VECTOR_ELT(ans, 1, dist);
+    int rc = icnv_knn_rows_f64(REAL(x), n, G, k, INTEGER(idx), REAL(dist));
+    if (rc == 0) {
+        int *p = INTEGER(idx);
+        for (int64_t e = 0; e < n * (int64_t)k; ++e) p[e] += 1;
+    }
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* normalize_counts_by_seq_depth (ops.R:3064-3111); normalize_factor NA -> median of colSums */
 SEXP icnvR_normalize(SEXP expr, SEXP normalize_factor) {
     SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
@@ -434,6 +457,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_clear_noise_threshold", (DL_FUNC)&icnvR_clear_noise_threshold, 4},
     {"icnvR_smooth_hmm", (DL_FUNC)&icnvR_smooth_hmm, 11},   {"icnvR_init_devices", (DL_FUNC)&icnvR_init_devices, 1},
     {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1}, {"icnvR_hclust", (DL_FUNC)&icnvR_hclust, 2},
+    {"icnvR_knn", (DL_FUNC)&icnvR_knn, 2},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -660,6 +660,19 @@ def parallelDist(x, method: str = "euclidean", threads=None) -> np.ndarray:
     return api.pairwise_dist_rows(x)
 
 
+def nn2(data, k=None) -> dict:
+    """`nn2(data, k = k)` as .leiden_simple_snn calls it (RANN::nn2, imported by the reference;
+    R/inferCNV_tumor_subclusters.R:725-741) on observations x variables `data`, the query set being the data set: RANN's
+    result, {"nn.idx": n x k 1-based, "nn.dists": n x k}, exact.  k defaults to min(10, nrow(data)) as in RANN."""
+    data = np.asarray(data, dtype=np.float64)
+    if data.ndim != 2:
+        raise ValueError("data must be a matrix (observations x variables)")
+    if k is None:
+        k = min(10, data.shape[0])
+    idx, dist = api.knn_rows(data, k)
+    return {"nn.idx": idx + 1, "nn.dists": dist}
+
+
 def hclust(d, method: str = "complete", members=None) -> dict:
     """`hclust(d, method)` as infercnv calls it (fastcluster::hclust, imported by the reference; R/inferCNV_ops.R:262 passes
     "ward.D2" by default) on a "dist" vector such as parallelDist()'s.  Returns a dict shaped like R's "hclust" object:
