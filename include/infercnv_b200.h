@@ -276,6 +276,39 @@ ICNV_API int icnv_hclust_f64(const double *d, int64_t n, int method, int32_t *me
  * Host only, no GPU. */
 ICNV_API int icnv_hclust_order(const int32_t *merge, int64_t n, int32_t *order);
 
+/* caTools::runmean(x, k) with its defaults (alg "C", endrule "mean", align "center") down every column of the G x C matrix X,
+ * per row range - smooth_by_chromosome_runmeans (R/inferCNV_ops.R:2679-2704) with the chromosomes as ranges.  For a range
+ * of L genes, k' = min(k, L), k2 = k' / 2, k1 = k' - 1 - k2: Y[p] = mean(X[max(0, p - k1) .. min(L - 1, p + k2)]) (positions
+ * within the range).  k <= 1, ranges of fewer than 2 genes and the genes outside every range are copied.  The K ranges
+ * (chr_start, chr_len; chr_start NULL: the single range [0, G), K ignored) must be ordered and disjoint inside [0, G).
+ * An even k is computed by the rule above.  Double-double running sum: |Y[p] - m| <= 2 u |m| + 8 L u^2 T / cnt
+ * (m the exact window mean, cnt its count, T the sum of |x| over the range, u = 2^-53), independent of the launch geometry.
+ * NaN / Inf anywhere in X: ICNV_E_NONFINITE (caTools skips NaNs; the R wrapper falls back). */
+ICNV_API int icnv_runmean_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *chr_start,
+                              const int32_t *chr_len, int K, int k);
+
+/* The permutation null of random-trees subclustering, .parameterize_random_cluster_heights_smoothed_trees
+ * (R/inferCNV_tumor_subclusters.random_smoothed_trees.R:217-304), for one clade in one call.  The clade is the list of n
+ * 0-based columns `cells` of the G x C matrix X (NULL: all C columns, n is then ignored).
+ *   Observed tree: icnv_runmean_f64(window) over [0, G) -> icnv_center_f64 (median) -> icnv_pairwise_dist_f64 ->
+ *   icnv_hclust_f64(method): merge / height / order exactly as that composition returns them, bit for bit.
+ *   perm_max_height[p], p < n_perm: the largest height of the tree built the same way on permutation p, which shuffles
+ *   every gene independently across the cells: key(p, g, i) = mix64(hash3(seed, p, g, i)) (the splitmix generator of
+ *   icnv_synth.cu, finalised once more so that the keys of one (p, g) order the positions uniformly),
+ *   pi_{p,g} = the stable ascending argsort of the keys over the list positions i, and
+ *   X_p[g, i] = X[g, cells[pi_{p,g}(i)]].  Member p depends only on (data, seed, p): the first m maxima of a call equal an
+ *   m-permutation call with the same seed.
+ * The members run in waves of B = min(n_perm + 1, SM count, members that fit the free device memory) linkages, one SM each;
+ * the result does not depend on B.  Device memory: the input, two G x n working copies and one n x n matrix per member of a
+ * wave.  Methods as icnv_hclust_f64.  n < 2, another method code or n_perm < 0: ICNV_E_BAD_ARG; centroid / median or
+ * n > 65536: ICNV_E_UNSUPPORTED; NaN / Inf in the clade: ICNV_E_NONFINITE; not even one member fits: ICNV_E_NOMEM. */
+ICNV_API int icnv_random_tree_heights_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int window,
+                                          int method, int n_perm, uint64_t seed, int32_t *merge, double *height,
+                                          int32_t *order, double *perm_max_height);
+/* What the last random-trees call did: out5 = {B, waves, ms of shuffle + runmean + centring, ms of distances, ms of
+ * linkages} (device time summed over the waves); zeros before any call. */
+ICNV_API int icnv_debug_random_trees(double *out5);
+
 /* Combine per-cell (sum, sd) pairs - e.g. all-gathered from several GPUs - into mu / sigma over all values
  * of those cells, in list order (what icnv_mean_sd_f64 does internally). */
 ICNV_API void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, int64_t G, double *mu,
@@ -450,6 +483,12 @@ ICNV_API int icnv_dev_knn_f64(const double *X, int64_t G, int64_t ldx, const int
  * copy of merge).  Synchronises the stream once, after filling the matrix, to report non-finite input; the linkage itself
  * is enqueued on `stream`. */
 ICNV_API int icnv_dev_hclust_f64(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream);
+/* icnv_random_tree_heights_f64 on device pointers: columns X + ldx * (d_cells ? d_cells[i] : i), i < n; merge / height /
+ * perm_max_height (device), no order (icnv_hclust_order on the host copy of merge).  Synchronises `stream` once, after the
+ * first wave's distances, to report non-finite input, and once at the end. */
+ICNV_API int icnv_dev_random_tree_heights_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
+                                              int window, int method, int n_perm, uint64_t seed, int32_t *merge,
+                                              double *height, double *perm_max_height, void *stream);
 /* Region calling on device-resident states (uint8, column stride lds >= G).
  * icnv_dev_state_counts_u8: counts[(k*G + g)*8 + slot] = number of cells of group k (d_cells[h_grp_off[k] ..
  * h_grp_off[k+1]), device) whose state at gene g falls in `slot` (0: unassigned, v+1: state v); integer counts, so

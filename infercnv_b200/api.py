@@ -382,6 +382,51 @@ def hclust_order(merge) -> np.ndarray:
     return order
 
 
+def runmean(X, k, chr_start=None, chr_len=None) -> np.ndarray:
+    """caTools::runmean(x, k) (endrule "mean", align "center") down every column of the genes x cells matrix X, per row
+    range (default: the whole column): smooth_by_chromosome_runmeans with the chromosomes as ranges.  Genes outside every
+    range, ranges of fewer than 2 genes and k <= 1 are copied (icnv_runmean_f64)."""
+    X = _f64(X)
+    G, C = X.shape
+    Y = np.empty_like(X, order="F")
+    if chr_start is None:
+        _lib.check(_lib.load().icnv_runmean_f64(_p(X), _p(Y), G, C, None, None, 0, int(k)))
+    else:
+        cs, cl = _i32(chr_start), _i32(chr_len)
+        if len(cs) != len(cl):
+            raise ValueError("chr_start and chr_len differ in length")
+        _lib.check(_lib.load().icnv_runmean_f64(_p(X), _p(Y), G, C, _p(cs), _p(cl), len(cs), int(k)))
+    return Y
+
+
+def random_tree_heights(X, window=101, method="ward.D2", n_perm=100, seed=0, cells=None):
+    """The permutation null of random-trees subclustering for the clade X[:, cells] (default: all columns) of the genes x
+    cells matrix X: (merge, height, order, perm_max).  merge / height / order are the observed tree, runmean(window) ->
+    median centring -> Euclidean distances -> hclust(method), as hclust() returns it; perm_max (n_perm) holds the largest
+    height of each permuted tree (every gene shuffled across the cells by the generator of icnv_random_tree_heights_f64)."""
+    X = _f64(X)
+    G, C = X.shape
+    idx = None if cells is None else _i32(cells)
+    n = C if idx is None else len(idx)
+    nm = max(n - 1, 0)
+    merge = np.empty((nm, 2), dtype=np.int32, order="F")
+    height = np.empty(nm, dtype=np.float64)
+    order = np.empty(max(n, 1), dtype=np.int32)
+    perm_max = np.empty(max(int(n_perm), 0), dtype=np.float64)
+    _lib.check(_lib.load().icnv_random_tree_heights_f64(
+        _p(X), G, C, _p(idx) if idx is not None else None, n, int(window), hclust_method_code(method), int(n_perm),
+        int(seed) & 0xFFFFFFFFFFFFFFFF, _p(merge), _p(height), _p(order), _p(perm_max) if perm_max.size else None))
+    return merge, height, order[:n], perm_max
+
+
+def random_trees_stats() -> dict:
+    """What the last random_tree_heights call did: the wave size B, the number of waves and the device time (ms) of its
+    stages (icnv_debug_random_trees)."""
+    out = np.zeros(5, dtype=np.float64)
+    _lib.check(_lib.load().icnv_debug_random_trees(_p(out)))
+    return {"B": int(out[0]), "waves": int(out[1]), "prep_ms": out[2], "dist_ms": out[3], "link_ms": out[4]}
+
+
 # ---- CNV region calling on the state matrix (R/inferCNV_HMM.R:706-1087) ---------------------------------------
 
 def _u8(a) -> np.ndarray:

@@ -1875,3 +1875,94 @@ int icnv_hclust_order(const int32_t *merge, int64_t n, int32_t *order) {
 }
 
 }  // extern "C"
+
+// ---- running means and the random-trees null (kernels and the device body in icnv_random_trees.cu) -------------------------
+// Weak references, as for the linkage: a build without icnv_random_trees.cu reports them as unsupported.
+namespace icnv {
+int runmean_launch(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t ncols, const int32_t *d_rs,
+                   const int32_t *d_rl, int K, int k, int *flag, cudaStream_t st) __attribute__((weak));
+int random_trees_dev(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int window, int method,
+                     int n_perm, unsigned long long seed, int32_t *merge, double *height, double *perm_max, void *stream,
+                     const char *who) __attribute__((weak));
+void random_trees_stats(double *out5) __attribute__((weak));
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_runmean_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len,
+                     int K, int k) {
+    if (!icnv::runmean_launch) return set_error(ICNV_E_UNSUPPORTED, "icnv_runmean_f64: this build has no running-mean kernel");
+    ICNV_HOST_PROLOGUE();
+    if (!X || !Y || G <= 0 || C <= 0 || (chr_start && (!chr_len || K < 0)))
+        return set_error(ICNV_E_BAD_ARG, "icnv_runmean_f64: bad argument");
+    if (!chr_start) K = 1;
+    for (int r = 0; chr_start && r < K; ++r) {   // ranges in order, disjoint, inside [0, G)
+        const int64_t prev_end = r ? (int64_t)chr_start[r - 1] + chr_len[r - 1] : 0;
+        if (chr_len[r] < 0 || chr_start[r] < prev_end || (int64_t)chr_start[r] + chr_len[r] > G)
+            return set_error(ICNV_E_BAD_ARG, "icnv_runmean_f64: range %d [%d, +%d) is not ordered and disjoint inside [0, %lld)",
+                             r, chr_start[r], chr_len[r], (long long)G);
+    }
+    int rc;
+    double *dX = nullptr, *dY = (double *)scratch(SLOT_OUT, sizeof(double) * (size_t)(G * C));
+    int32_t *d_r = (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * 2 * (size_t)K + 16);
+    int *d_flag = (int *)scratch(SLOT_MISC, 64);
+    if (!dY || !d_r || !d_flag) return ICNV_E_NOMEM;
+    if ((rc = upload_matrix(X, G * C, &dX, SLOT_IN, st))) return rc;
+    ICNV_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
+    if (chr_start) {
+        ICNV_CUDA(cudaMemcpyAsync(d_r, chr_start, sizeof(int32_t) * (size_t)K, cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaMemcpyAsync(d_r + K, chr_len, sizeof(int32_t) * (size_t)K, cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = icnv::runmean_launch(dX, G, dY, G, G, C, chr_start ? d_r : nullptr, chr_start ? d_r + K : nullptr, K, k, d_flag, st)))
+        return rc;
+    ICNV_CUDA(cudaMemcpyAsync(Y, dY, sizeof(double) * (size_t)(G * C), cudaMemcpyDeviceToHost, st));
+    return check_flag(d_flag, st);
+}
+
+int icnv_dev_random_tree_heights_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int window,
+                                     int method, int n_perm, uint64_t seed, int32_t *merge, double *height, double *perm_max,
+                                     void *stream) {
+    if (!icnv::random_trees_dev)
+        return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_random_tree_heights_f64: this build has no random-trees kernels");
+    return icnv::random_trees_dev(X, G, ldx, d_cells, n, window, method, n_perm, seed, merge, height, perm_max, stream,
+                                  "icnv_dev_random_tree_heights_f64");
+}
+
+int icnv_random_tree_heights_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int window,
+                                 int method, int n_perm, uint64_t seed, int32_t *merge, double *height, int32_t *order,
+                                 double *perm_max) {
+    if (!icnv::random_trees_dev)
+        return set_error(ICNV_E_UNSUPPORTED, "icnv_random_tree_heights_f64: this build has no random-trees kernels");
+    ICNV_HOST_PROLOGUE();
+    if (!cells) n = C;
+    if (!X || G <= 0 || C <= 0 || !merge || !height || !order || (n_perm > 0 && !perm_max))
+        return set_error(ICNV_E_BAD_ARG, "icnv_random_tree_heights_f64: bad argument");
+    for (int64_t i = 0; cells && i < n; ++i)
+        if (cells[i] < 0 || cells[i] >= C) return set_error(ICNV_E_BAD_ARG, "icnv_random_tree_heights_f64: cell index out of range");
+    const int64_t nm = n > 1 ? n - 1 : 0, np = n_perm > 0 ? n_perm : 0;
+    int rc;
+    double *dX = nullptr, *d_out = (double *)scratch(SLOT_OUT, sizeof(double) * (size_t)(nm + np) + sizeof(int32_t) * 2 * (size_t)nm);
+    int32_t *d_idx = cells ? (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * (size_t)std::max<int64_t>(n, 1)) : nullptr;
+    if (!d_out || (cells && !d_idx)) return ICNV_E_NOMEM;
+    if ((rc = upload_matrix(X, G * C, &dX, SLOT_IN, st))) return rc;
+    if (cells && n > 0) ICNV_CUDA(cudaMemcpyAsync(d_idx, cells, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    double *d_height = d_out, *d_perm = d_out + nm;
+    int32_t *d_merge = (int32_t *)(d_perm + np);
+    if ((rc = icnv::random_trees_dev(dX, G, G, d_idx, n, window, method, n_perm, seed, d_merge, d_height, d_perm, st,
+                                     "icnv_random_tree_heights_f64")))
+        return rc;
+    ICNV_CUDA(cudaMemcpyAsync(height, d_height, sizeof(double) * (size_t)nm, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaMemcpyAsync(merge, d_merge, sizeof(int32_t) * 2 * (size_t)nm, cudaMemcpyDeviceToHost, st));
+    if (np) ICNV_CUDA(cudaMemcpyAsync(perm_max, d_perm, sizeof(double) * (size_t)np, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return icnv_hclust_order(merge, n, order);
+}
+
+int icnv_debug_random_trees(double *out5) {
+    if (!out5) return set_error(ICNV_E_BAD_ARG, "icnv_debug_random_trees: out5 is NULL");
+    for (int i = 0; i < 5; ++i) out5[i] = 0.0;
+    if (icnv::random_trees_stats) icnv::random_trees_stats(out5);
+    return ICNV_OK;
+}
+
+}  // extern "C"

@@ -159,6 +159,17 @@ __device__ __forceinline__ double double_of_key(unsigned long long k) {
     return __longlong_as_double((long long)u);
 }
 
+// Counter-based splitmix64 generator: a pure function of its arguments (the synthetic workload, the permutations of the
+// random-trees null).  oracle/infercnv_oracle.c (syn_hash3) and tests/runmean_reference.py restate it.
+__device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser
+    z += 0x9e3779b97f4a7c15ull;
+    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+    return z ^ (z >> 31);
+}
+__device__ __forceinline__ uint64_t hash3(uint64_t seed, uint64_t a, uint64_t b, uint64_t c) {
+    return mix64(mix64(mix64(seed ^ 0x243f6a8885a308d3ull) + a) * 0x9fb21c651e98df25ull + b) ^ mix64(c + 0x13198a2e03707344ull);
+}
 __device__ __forceinline__ double warp_min_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));

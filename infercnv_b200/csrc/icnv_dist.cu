@@ -154,6 +154,66 @@ __global__ void __launch_bounds__(PD_NT, 1) pairwise_dist_kernel(const DistParam
     }
 }
 
+// ---- K13b's distances: pairwise_dist_kernel's tiles written straight into the linkage's square matrices -----------------
+// Member z = blockIdx.x / T (tile column blockIdx.x % T, T tiles per side): columns X + z * sx (ldx, no cell list), matrix M + z * sm (n x ld).  Entry (a, b), a != b, is the
+// value hclust_fill_kernel would store from pairwise_dist_kernel's entry of the pair, v = sqrt(sum) (v * v for ward.D2), in
+// both triangles; the diagonal is +inf.  flag |= 1 when a value is not finite, as that kernel reports it.
+struct DistSqParams {
+    DistParams d;         // X, G, ldx, n, rows = 0, cells = out = nullptr
+    int64_t sx, sm, ld;
+    unsigned T;
+    double *M;
+    int square;
+    int *flag;
+};
+
+__global__ void __launch_bounds__(PD_NT, 1) dist_square_kernel(const DistSqParams q) {
+    const unsigned z = blockIdx.x / q.T;
+    const int bi = blockIdx.y, bj = (int)(blockIdx.x - z * q.T);
+    if (bi > bj) return;
+    extern __shared__ __align__(16) double pd_smem[];
+    double *As = pd_smem;
+    double *Bs = pd_smem + 2 * PD_T * PD_LD;
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int64_t i0 = (int64_t)bi * PD_T, j0 = (int64_t)bj * PD_T, n = q.d.n, ld = q.ld;
+    DistParams p = q.d;
+    p.X += (int64_t)z * q.sx;
+    double *M = q.M + (int64_t)z * q.sm;
+    double acc[8][8];
+    dist_tile(p, i0, j0, As, Bs, acc);
+    bool bad = false;
+#pragma unroll
+    for (int pp = 0; pp < 8; ++pp) {
+        const int64_t a = i0 + ty + 16 * pp;
+        if (a >= n) continue;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const int64_t b = j0 + tx + 16 * c;
+            if (b == a) M[a * ld + a] = __longlong_as_double(0x7ff0000000000000ll);
+            if (b <= a || b >= n) continue;
+            const double v = sqrt(acc[pp][c]);
+            bad |= !is_finite_d(v);
+            const double w = q.square ? __dmul_rn(v, v) : v;
+            M[a * ld + b] = w;
+            M[b * ld + a] = w;
+        }
+    }
+    if (bad) atomicOr(q.flag, 1);
+}
+
+// B members of n cells each (genes x cells, member z's columns at X + z * sx) -> their n x ld matrices (M + z * sm)
+int dist_square_launch(const double *X, int64_t G, int64_t ldx, int64_t sx, int64_t n, int B, double *M, int64_t ld,
+                       int64_t sm, int square, int *flag, cudaStream_t st) {
+    const int64_t T = (n + PD_T - 1) / PD_T;
+    if (T > 65535) return set_error(ICNV_E_UNSUPPORTED, "distances: %lld cells (limit %d)", (long long)n, 65535 * PD_T);
+    DistSqParams q{{X, G, ldx, nullptr, n, nullptr, 0}, sx, sm, ld, (unsigned)T, M, square, flag};
+    const size_t smem = sizeof(double) * 4 * PD_T * PD_LD;
+    ICNV_CUDA(cudaFuncSetAttribute(dist_square_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dist_square_kernel<<<dim3((unsigned)(T * B), (unsigned)T), PD_NT, smem, st>>>(q);
+    ICNV_CHECK_LAUNCH("dist_square_kernel");
+    return ICNV_OK;
+}
+
 // ---- K12: exact k nearest neighbours (RANN::nn2(data, k = k) with the query set = the data set) --------------------------
 //
 // Order: ascending squared distance, then ascending list position - a total order, so the result does not depend on launch

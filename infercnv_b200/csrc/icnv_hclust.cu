@@ -86,6 +86,9 @@ struct HcParams {
     int32_t *merge;          // (n - 1) x 2, column-major
     double *height;          // n - 1
     int P;
+    // a batched launch runs one linkage per CTA: member z = blockIdx.x works on M + z sM, raw_h / skey + z s8,
+    // chain .. sidx + z s4, merge + z 2 (n - 1) and height + z (n - 1)
+    int64_t sM, s8, s4;
 };
 
 __device__ __forceinline__ double lance_williams(int method, double dki, double dkj, double dij, double ni, double nj,
@@ -142,7 +145,23 @@ __global__ void __launch_bounds__(256) hclust_mirror_kernel(double *M, int64_t n
     }
 }
 
-__global__ void __launch_bounds__(HC_NT, 1) hclust_nn_chain_kernel(const HcParams p) {
+__global__ void __launch_bounds__(HC_NT, 1) hclust_nn_chain_kernel(const HcParams p0) {
+    HcParams p = p0;
+    {
+        const int64_t z = blockIdx.x;
+        p.M += z * p0.sM;
+        p.raw_h += z * p0.s8;
+        p.skey += z * p0.s8;
+        p.chain += z * p0.s4;
+        p.size += z * p0.s4;
+        p.raw_i += z * p0.s4;
+        p.raw_j += z * p0.s4;
+        p.uf += z * p0.s4;
+        p.node += z * p0.s4;
+        p.sidx += z * p0.s4;
+        p.merge += z * 2 * (p0.n - 1);
+        p.height += z * (p0.n - 1);
+    }
     extern __shared__ __align__(16) unsigned char hc_smem[];
     double *buf = reinterpret_cast<double *>(hc_smem);                    // [HC_S][HC_CH]
     unsigned char *active = hc_smem + sizeof(double) * HC_S * HC_CH;      // [n]
@@ -330,7 +349,7 @@ namespace icnv {
 using namespace hc;
 
 // Checks shared by the entry points; ICNV_OK when the linkage can run.
-static int hclust_check_args(int64_t n, int method, const char *who) {
+int hclust_check_args(int64_t n, int method, const char *who) {
     if (n < 2) return set_error(ICNV_E_BAD_ARG, "%s: n = %lld (at least 2 observations)", who, (long long)n);
     if (method == 5 || method == 6)
         return set_error(ICNV_E_UNSUPPORTED, "%s: method %d (centroid / median) is not reducible", who, method);
@@ -340,7 +359,7 @@ static int hclust_check_args(int64_t n, int method, const char *who) {
 }
 
 // The square matrix of n observations: n x ld doubles, ld = n rounded up to even.
-static int64_t hclust_ld(int64_t n) { return (n + 1) & ~(int64_t)1; }
+int64_t hclust_ld(int64_t n) { return (n + 1) & ~(int64_t)1; }
 
 // Fill rows [a0, a1) of M from the condensed entries of those rows in src (device), flag |= 1 on a non-finite entry.
 static int hclust_fill_rows(const double *src, int64_t a0, int64_t a1, int64_t n, int method, double *M, int *flag,
@@ -353,20 +372,16 @@ static int hclust_fill_rows(const double *src, int64_t a0, int64_t a1, int64_t n
     return ICNV_OK;
 }
 
-// Mirror the upper triangle, check the flag (one synchronisation), then enqueue the linkage.  M is freed on `st` after it.
-static int hclust_run(double *M, int64_t n, int method, int *d_flag, int32_t *merge, double *height, cudaStream_t st) {
+// B linkages of n observations in one launch, one CTA (one SM) each: member z's filled matrix (symmetric, diagonal +inf,
+// squared for ward.D2) at M + z n ld, its merge / height at merge + z 2 (n - 1) / height + z (n - 1).  Every member is
+// the same function of its own matrix as a single-tree launch (B = 1).  The scratch is freed on `st` after the launch.
+int hclust_batch(double *M, int64_t n, int method, int B, int32_t *merge, double *height, cudaStream_t st) {
     const int64_t ld = hclust_ld(n);
-    const unsigned T = (unsigned)((n + 31) / 32);
-    hclust_mirror_kernel<<<dim3(T, T), 256, 0, st>>>(M, n, ld);
-    ICNV_CHECK_LAUNCH("hclust_mirror_kernel");
-    int h_flag = 0;
-    ICNV_CUDA(cudaMemcpyAsync(&h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    ICNV_CUDA(cudaStreamSynchronize(st));
-    if (h_flag) return set_error(ICNV_E_NONFINITE, "hclust: NaN or Inf in the dissimilarities");
     int P = 1;
     while (P < n - 1) P <<= 1;
-    // scratch of the linkage: chain, size, raw_i, raw_j, uf, node, sidx (int32) and raw_h, skey (8 bytes)
-    const size_t b8 = sizeof(double) * ((size_t)n + (size_t)P), b4 = sizeof(int32_t) * (6 * (size_t)n + (size_t)P);
+    // scratch of a linkage: chain, size, raw_i, raw_j, uf, node, sidx (int32) and raw_h, skey (8 bytes)
+    const int64_t s8 = n + P, s4 = 6 * n + P;
+    const size_t b8 = sizeof(double) * (size_t)s8 * (size_t)B, b4 = sizeof(int32_t) * (size_t)s4 * (size_t)B;
     char *w = nullptr;
     ICNV_CUDA(cudaMallocAsync((void **)&w, b8 + b4 + 64, st));
     HcParams q;
@@ -387,12 +402,35 @@ static int hclust_run(double *M, int64_t n, int method, int *d_flag, int32_t *me
     q.merge = merge;
     q.height = height;
     q.P = P;
+    q.sM = n * ld;
+    q.s8 = s8;
+    q.s4 = s4;
     const size_t smem = sizeof(double) * HC_S * HC_CH + (size_t)((n + 15) & ~15);
     ICNV_CUDA(cudaFuncSetAttribute(hclust_nn_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    hclust_nn_chain_kernel<<<1, HC_NT, smem, st>>>(q);
+    hclust_nn_chain_kernel<<<B, HC_NT, smem, st>>>(q);
     ICNV_CHECK_LAUNCH("hclust_nn_chain_kernel");
     ICNV_CUDA(cudaFreeAsync(w, st));
     return ICNV_OK;
+}
+
+// Bytes of device scratch hclust_batch allocates per member.
+size_t hclust_batch_scratch(int64_t n) {
+    int64_t P = 1;
+    while (P < n - 1) P <<= 1;
+    return sizeof(double) * (size_t)(n + P) + sizeof(int32_t) * (size_t)(6 * n + P);
+}
+
+// Mirror the upper triangle, check the flag (one synchronisation), then enqueue the linkage.  M is freed on `st` after it.
+static int hclust_run(double *M, int64_t n, int method, int *d_flag, int32_t *merge, double *height, cudaStream_t st) {
+    const int64_t ld = hclust_ld(n);
+    const unsigned T = (unsigned)((n + 31) / 32);
+    hclust_mirror_kernel<<<dim3(T, T), 256, 0, st>>>(M, n, ld);
+    ICNV_CHECK_LAUNCH("hclust_mirror_kernel");
+    int h_flag = 0;
+    ICNV_CUDA(cudaMemcpyAsync(&h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    if (h_flag) return set_error(ICNV_E_NONFINITE, "hclust: NaN or Inf in the dissimilarities");
+    return hclust_batch(M, n, method, 1, merge, height, st);
 }
 
 }  // namespace icnv

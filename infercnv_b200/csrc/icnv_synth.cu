@@ -13,15 +13,6 @@
 
 namespace icnv {
 
-__device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser
-    z += 0x9e3779b97f4a7c15ull;
-    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-    return z ^ (z >> 31);
-}
-__device__ __forceinline__ uint64_t hash3(uint64_t seed, uint64_t a, uint64_t b, uint64_t c) {
-    return mix64(mix64(mix64(seed ^ 0x243f6a8885a308d3ull) + a) * 0x9fb21c651e98df25ull + b) ^ mix64(c + 0x13198a2e03707344ull);
-}
 __device__ __forceinline__ double u01(uint64_t h) {  // (0, 1]
     return ((double)(h >> 11) + 1.0) * (1.0 / 9007199254740992.0);
 }

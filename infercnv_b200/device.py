@@ -425,6 +425,27 @@ class Engine:
         m = merge.cpu().numpy().T
         return m, height.cpu().numpy(), hclust_order(m)
 
+    def random_tree_heights(self, X, cells=None, window=101, method="ward.D2", n_perm=100, seed=0):
+        """The random-trees permutation null of the clade `cells` (rows of the resident (C, G) float64 tensor X with
+        contiguous genes; default all) on the device: (merge, height, order, perm_max) as numpy arrays, as
+        api.random_tree_heights returns them.  Nothing but the cell list goes up and the results come back."""
+        from .api import hclust_method_code, hclust_order
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        G = X.shape[1]
+        idx = None if cells is None else torch.as_tensor(np.asarray(cells, dtype=np.int32), device=self.tdev)
+        n = X.shape[0] if idx is None else int(idx.numel())
+        nm = max(n - 1, 0)
+        merge = torch.empty((2, nm), dtype=torch.int32, device=self.tdev)   # column-major (n - 1) x 2
+        height = torch.empty(nm, dtype=torch.float64, device=self.tdev)
+        perm_max = torch.empty(max(int(n_perm), 0), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_random_tree_heights_f64(
+            X.data_ptr(), G, max(X.stride(0), G), idx.data_ptr() if idx is not None else None, n, int(window),
+            hclust_method_code(method), int(n_perm), int(seed) & 0xFFFFFFFFFFFFFFFF, merge.data_ptr(), height.data_ptr(),
+            perm_max.data_ptr() if perm_max.numel() else None, _stream_ptr()))
+        m = merge.cpu().numpy().T
+        return m, height.cpu().numpy(), hclust_order(m), perm_max.cpu().numpy()
+
     def mean_sd(self, X, groups_local):
         """mu / sigma over all values of the listed cells across ALL ranks (.i3HMM_get_sd_trend_by_num_cells_fit,
         R/inferCNV_i3HMM.R:17-30).  groups_local: per group, this rank's LOCAL columns (the planner's slices).

@@ -503,6 +503,68 @@ b200_nn2 <- function(data, query = data, k = min(10, nrow(data)), treetype = c("
     orig(data, query = query, k = k, treetype = treetype, searchtype = searchtype, radius = radius, eps = eps)
 }
 
+## smooth_by_chromosome_runmeans (R/inferCNV_ops.R:2679-2704), run()'s step 10 for smooth_method = "runmeans":
+## apply(chr_data, 2, caTools::runmean, k = window_length) per chromosome, chromosomes of one gene left alone, hspike
+## mirrored.  Falls back for NA, an even window, a non-double / non-matrix slot, genes of a chromosome not contiguous, or a
+## library error.
+b200_smooth_by_chromosome_runmeans <- function(infercnv_obj, window_length) {
+    orig <- .icnv_env$orig$smooth_by_chromosome_runmeans
+    m <- infercnv_obj@expr.data
+    codes <- .icnv_chr_codes(infercnv_obj)
+    if (!.icnv_enabled() || !.icnv_ok(m) || is.null(codes) || !is.numeric(window_length) || length(window_length) != 1 ||
+        is.na(window_length) || window_length %% 2 == 0)
+        return(orig(infercnv_obj, window_length))
+    r <- rle(codes)
+    lens <- as.integer(r$lengths)
+    starts <- as.integer(c(0L, cumsum(lens)[-length(lens)]))
+    for (chr in unique(infercnv_obj@gene_order[["chr"]])) futile.logger::flog.info(paste0("smooth_by_chromosome: chr: ", chr))
+    res <- .icnv_try(.Call("icnvR_runmean", m, starts, lens, as.integer(window_length)), "smooth_by_chromosome_runmeans")
+    if (is.null(res)) return(orig(infercnv_obj, window_length))
+    dimnames(res) <- dimnames(m)
+    infercnv_obj@expr.data <- res
+    if (!is.null(infercnv_obj@.hspike)) {
+        futile.logger::flog.info("-mirroring for hspike")
+        infercnv_obj@.hspike <- b200_smooth_by_chromosome_runmeans(infercnv_obj@.hspike, window_length)
+    }
+    infercnv_obj
+}
+
+## .parameterize_random_cluster_heights_smoothed_trees (R/inferCNV_tumor_subclusters.random_smoothed_trees.R:217-304): the
+## observed tree and the 100 permuted maxima of one clade in one GPU call, the same list(h_obs, max_h,
+## rand_max_height_dist, ecdf).  h_obs is the "hclust" object b200_hclust returns (labels = colnames(expr_matrix)).  The
+## permutations come from the library's generator, seeded by two draws of R's RNG, so set.seed() before run() makes the
+## null reproducible; the distribution is R's sample(), the draws are not.  Falls back for methods outside the six,
+## n outside [2, 65536], NA, or a library error.
+b200_.parameterize_random_cluster_heights_smoothed_trees <- function(expr_matrix, hclust_method, window_size, plot = FALSE) {
+    orig <- .icnv_env$orig$.parameterize_random_cluster_heights_smoothed_trees
+    codes <- c(single = 0L, complete = 1L, average = 2L, mcquitty = 3L, ward.D = 4L, ward.D2 = 7L)
+    n <- if (is.matrix(expr_matrix)) ncol(expr_matrix) else NA
+    ok <- .icnv_enabled() && .icnv_ok(expr_matrix) && is.character(hclust_method) && length(hclust_method) == 1 &&
+        hclust_method %in% names(codes) && !is.na(n) && n >= 2 && n <= 65536 && is.numeric(window_size) &&
+        length(window_size) == 1 && !is.na(window_size)
+    if (ok) {
+        seed <- as.double(c(sample.int(2^31 - 1, 1), sample.int(2^31 - 1, 1)))
+        res <- .icnv_try(.Call("icnvR_random_tree_heights", expr_matrix, as.integer(window_size), codes[[hclust_method]],
+                               100L, seed), "random trees")
+        if (!is.null(res)) {
+            h_obs <- structure(list(merge = res[[1]], height = res[[2]], order = res[[3]], labels = colnames(expr_matrix),
+                                    method = hclust_method, call = match.call(), dist.method = "euclidean"),
+                               class = "hclust")
+            max_rand_heights <- res[[4]]
+            max_height <- max(h_obs$height)
+            message(sprintf("Lengths for original tree branches (h): %s", paste(h_obs$height, sep = ",", collapse = ",")))
+            message(sprintf("Max height: %g", max_height))
+            message(sprintf("Lengths for max heights: %s", paste(max_rand_heights, sep = ",", collapse = ",")))
+            e <- stats::ecdf(max_rand_heights)
+            message(sprintf("pval: %g", 1 - e(max_height)))
+            params_list <- list(h_obs = h_obs, max_h = max_height, rand_max_height_dist = max_rand_heights, ecdf = e)
+            if (plot) infercnv:::.plot_tree_height_dist(params_list)
+            return(params_list)
+        }
+    }
+    orig(expr_matrix, hclust_method, window_size, plot)
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -510,7 +572,9 @@ infercnvb200_install <- function() {
              "apply_median_filtering", "normalize_counts_by_seq_depth", "clear_noise_via_ref_mean_sd",
              "get_predicted_CNV_regions", "remove_outliers_norm", "clear_noise",
              "predict_CNV_via_HMM_on_tumor_subclusters_per_chr", "i3HMM_predict_CNV_via_HMM_on_tumor_subclusters",
-             "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr")
+             "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
+             ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
+             ".parameterize_random_cluster_heights_smoothed_trees")
     ns <- asNamespace("infercnv")
     .icnv_env$orig <- lapply(stats::setNames(fns, fns), function(f) get(f, envir = ns))
     for (f in fns) utils::assignInNamespace(f, get(paste0("b200_", f)), ns = "infercnv")

@@ -256,6 +256,46 @@ SEXP icnvR_hclust(SEXP d, SEXP method_code) {
     return ans;
 }
 
+/* apply(m, 2, caTools::runmean, k = k) per row range - smooth_by_chromosome_runmeans (ops.R:2679-2704) with the ranges the
+ * R closure computed (0-based starts, lengths; genes outside them are copied). */
+SEXP icnvR_runmean(SEXP expr, SEXP chr_start, SEXP chr_len, SEXP k) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int K = Rf_length(chr_start);
+    if (Rf_length(chr_len) != K) Rf_error("infercnv_b200: runmean ranges differ in length");
+    SEXP ans = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    int rc = icnv_runmean_f64(REAL(expr), REAL(ans), G, C, (const int32_t *)INTEGER(chr_start),
+                              (const int32_t *)INTEGER(chr_len), K, Rf_asInteger(k));
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
+/* .parameterize_random_cluster_heights_smoothed_trees (random_smoothed_trees.R:217-304) on the clade matrix expr (genes x
+ * cells): list(merge, height, order, rand_max_height_dist); the closure builds the "hclust" object.  seed: two whole numbers
+ * in [0, 2^31) drawn from R's RNG, combined as hi * 2^32 + lo. */
+SEXP icnvR_random_tree_heights(SEXP expr, SEXP window, SEXP method_code, SEXP n_perm, SEXP seed) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], n = INTEGER(dim)[1];
+    int np = Rf_asInteger(n_perm);
+    if (n < 2 || np < 0 || Rf_length(seed) != 2) Rf_error("infercnv_b200: random trees need 2 cells, n_perm >= 0, two seeds");
+    uint64_t sd = ((uint64_t)REAL(seed)[0] << 32) | (uint64_t)REAL(seed)[1];
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 4));
+    SEXP merge = Rf_allocMatrix(INTSXP, (int)(n - 1), 2);
+    SET_VECTOR_ELT(ans, 0, merge);
+    SEXP height = Rf_allocVector(REALSXP, (R_xlen_t)(n - 1));
+    SET_VECTOR_ELT(ans, 1, height);
+    SEXP order = Rf_allocVector(INTSXP, (R_xlen_t)n);
+    SET_VECTOR_ELT(ans, 2, order);
+    SEXP pm = Rf_allocVector(REALSXP, (R_xlen_t)np);
+    SET_VECTOR_ELT(ans, 3, pm);
+    int rc = icnv_random_tree_heights_f64(REAL(expr), G, n, NULL, n, Rf_asInteger(window), Rf_asInteger(method_code), np, sd,
+                                          INTEGER(merge), REAL(height), INTEGER(order), np > 0 ? REAL(pm) : NULL);
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* nn2(data, k = k) (RANN::nn2, an import of infercnv) with the query set = the data set, data = observations x variables
  * (.leiden_simple_snn, R/inferCNV_tumor_subclusters.R:725-741).  Returns list(nn.idx n x k INTSXP, 1-based, nn.dists n x k
  * REALSXP); the R closure names the fields. */
@@ -458,6 +498,8 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_smooth_hmm", (DL_FUNC)&icnvR_smooth_hmm, 11},   {"icnvR_init_devices", (DL_FUNC)&icnvR_init_devices, 1},
     {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1}, {"icnvR_hclust", (DL_FUNC)&icnvR_hclust, 2},
     {"icnvR_knn", (DL_FUNC)&icnvR_knn, 2},
+    {"icnvR_runmean", (DL_FUNC)&icnvR_runmean, 4},
+    {"icnvR_random_tree_heights", (DL_FUNC)&icnvR_random_tree_heights, 5},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -682,3 +682,24 @@ def hclust(d, method: str = "complete", members=None) -> dict:
         raise NotImplementedError("hclust(members=...) is not on the GPU path")
     merge, height, order = api.hclust(d, method)
     return {"merge": merge, "height": height, "order": order, "labels": None, "method": method, "dist.method": "euclidean"}
+
+
+def runmean(x, k) -> np.ndarray:
+    """`caTools::runmean(x, k)` with its defaults (endrule "mean", align "center") as infercnv applies it, column by
+    column (`apply(m, 2, caTools::runmean, k = k)`): a vector or a genes x cells matrix (icnv_runmean_f64)."""
+    x = np.asarray(x, dtype=np.float64)
+    if x.ndim == 1:
+        return api.runmean(x[:, None], k)[:, 0]
+    return api.runmean(x, k)
+
+
+def parameterize_random_cluster_heights_smoothed_trees(expr_matrix, hclust_method, window_size, n_perm=100, seed=0) -> dict:
+    """`.parameterize_random_cluster_heights_smoothed_trees(expr_matrix, hclust_method, window_size)`
+    (R/inferCNV_tumor_subclusters.random_smoothed_trees.R:217-304) on the genes x cells clade matrix: the reference's list
+    fields h_obs (as hclust() returns it), max_h and rand_max_height_dist (n_perm maxima, 100 in the reference).  The
+    permutations come from the library's own generator at `seed` - the same distribution as R's sample(), not its draws."""
+    merge, height, order, perm_max = api.random_tree_heights(expr_matrix, window=window_size, method=hclust_method,
+                                                             n_perm=n_perm, seed=seed)
+    h_obs = {"merge": merge, "height": height, "order": order, "labels": None, "method": hclust_method,
+             "dist.method": "euclidean"}
+    return {"h_obs": h_obs, "max_h": float(height.max()), "rand_max_height_dist": perm_max}
