@@ -309,6 +309,38 @@ ICNV_API int icnv_random_tree_heights_f64(const double *X, int64_t G, int64_t C,
  * linkages} (device time summed over the waves); zeros before any call. */
 ICNV_API int icnv_debug_random_trees(double *out5);
 
+/* mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52; run() step 21, R/inferCNV_ops.R:1509-1524) on the G x C matrix X:
+ * get_DE_genes_basic's tests, BH and .mask_DE_genes' mask in one call.
+ *   Groups (CSR, 0-based columns): n_ref >= 1 reference groups; n_sub >= 0 TESTED subclusters in R's loop order (observation
+ *   group by group, its subclusters in names() order - a group whose subclusters are not a named list is tested by R for
+ *   nothing and is simply not listed).  Pair column s * n_ref + j: x = reference group j, y = subcluster s.
+ *   test 0 (wilcoxon, :191-203): each side jittered (below), then wilcox.test(x, y) with R's defaults - exact when n_x < 50,
+ *        n_y < 50 and no ties in x u y, else the normal approximation with continuity and tie corrections (NaN when every
+ *        value of the pair is tied).  test 1 (t, :166-176): Welch's t.test(x, y) on the unjittered values; NaN where R's
+ *        try() catches an error (n < 2, or stderr < 10 eps max(|mean x|, |mean y|)).
+ *   p_adj: p.adjust(method = "BH") per pair over the genes in R's operation order, n = the non-NaN count; NaN stays NaN.
+ *   DE: p_adj < p_thresh.  Mask: per cell and gene a count - reference cells and the cells of a tested subcluster of < 5
+ *   list entries start at n_ref, each cell of a tested subcluster of >= 5 entries adds 1 per reference group where the gene
+ *   is DE for that subcluster (once per subcluster), other cells start at 0; rule 0 "any" masks count == 0, 1 "most"
+ *   count < n_ref / 2, 2 "all" count != n_ref.  Masked entries of Y are mask_val (R's center_val), the others X's.
+ *   Generator (Wilcoxon): jitter = jitter_mean + jitter_sd z (no contraction), z Box-Muller on two (0, 1] uniforms
+ *   ((mix64(hash3(seed, a, g, 2 i + k)) >> 11) + 1) 2^-53 (k = 0, 1), z = sqrt(-2 log u_0) cospi(2 u_1); g the gene, i the
+ *   list position within the group, a = j for reference group j, a = 2^32 + pair for a subcluster.  Reference-side draws
+ *   are keyed by (j, gene, position) and shared by all subclusters, so each reference row is jittered and sorted once per
+ *   gene: the joint law of one subcluster's columns equals R's (it uses each reference group once), but the columns of
+ *   different subclusters are dependent through the shared draws, where R's are conditionally independent.  R's closure
+ *   passes 1e-4 / 1e-4; jitter_sd = 0 keeps every tie and makes the statistic deterministic.
+ * Y (G x C; may be X), p_raw and p_adj (G x (n_sub n_ref), column-major, column s * n_ref + j) are each nullable.
+ * An empty group, an index out of range, an unknown test or rule code, jitter_sd < 0: ICNV_E_BAD_ARG; NaN / Inf in a listed
+ * cell: ICNV_E_NONFINITE; not enough device memory: ICNV_E_NOMEM. */
+ICNV_API int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *ref_off,
+                                  const int32_t *ref_idx, int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub,
+                                  int test, double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd,
+                                  uint64_t seed, double *p_raw, double *p_adj);
+/* What the last mask call did: out7 = {gene tiles, genes per tile, ms of (a) gather, (b) reference sorts / group statistics,
+ * (c) pair tests, (d) BH, (e) mask} (device time summed over the tiles); zeros before any call. */
+ICNV_API int icnv_debug_mask_non_de(double *out7);
+
 /* Combine per-cell (sum, sd) pairs - e.g. all-gathered from several GPUs - into mu / sigma over all values
  * of those cells, in list order (what icnv_mean_sd_f64 does internally). */
 ICNV_API void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, int64_t G, double *mu,
@@ -489,6 +521,14 @@ ICNV_API int icnv_dev_hclust_f64(const double *d_dist, int64_t n, int method, in
 ICNV_API int icnv_dev_random_tree_heights_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
                                               int window, int method, int n_perm, uint64_t seed, int32_t *merge,
                                               double *height, double *perm_max_height, void *stream);
+/* icnv_mask_non_de_f64 on device pointers: X (column stride ldx >= G), Y (ldy >= G; may be X, nullable), p_raw / p_adj
+ * (G x (n_sub n_ref), nullable); the group lists are HOST arrays.  Synchronises `stream` after each gene tile (non-finite
+ * check) and at the end. */
+ICNV_API int icnv_dev_mask_non_de_f64(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C,
+                                      const int32_t *ref_off /*host*/, const int32_t *ref_idx /*host*/, int n_ref,
+                                      const int32_t *sub_off /*host*/, const int32_t *sub_idx /*host*/, int n_sub, int test,
+                                      double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd,
+                                      uint64_t seed, double *p_raw, double *p_adj, void *stream);
 /* Region calling on device-resident states (uint8, column stride lds >= G).
  * icnv_dev_state_counts_u8: counts[(k*G + g)*8 + slot] = number of cells of group k (d_cells[h_grp_off[k] ..
  * h_grp_off[k+1]), device) whose state at gene g falls in `slot` (0: unassigned, v+1: state v); integer counts, so

@@ -427,6 +427,51 @@ def random_trees_stats() -> dict:
     return {"B": int(out[0]), "waves": int(out[1]), "prep_ms": out[2], "dist_ms": out[3], "link_ms": out[4]}
 
 
+DE_TESTS = {"wilcoxon": 0, "t": 1}
+DE_RULES = {"any": 0, "most": 1, "all": 2}
+
+
+def _code(table, v, what) -> int:
+    if isinstance(v, str):
+        if v not in table:
+            raise ValueError(f"unknown {what} {v!r}")
+        return table[v]
+    return int(v)
+
+
+def mask_non_de_genes(X, ref_groups, subclusters, test="wilcoxon", p_val_thresh=0.05, rule="any", center_val=None,
+                      jitter_mean=1e-4, jitter_sd=1e-4, seed=0, want_y=True):
+    """mask_non_DE_genes_basic on the genes x cells matrix X (icnv_mask_non_de_f64): ref_groups and subclusters are lists
+    of 0-based column lists, the subclusters the TESTED ones in R's loop order.  Returns (Y, p_raw, p_adj): Y the masked
+    matrix (None when want_y is False), p_raw / p_adj G x (len(subclusters) * len(ref_groups)), column s * n_ref + j.
+    center_val defaults to the mean of X, as in R."""
+    X = _f64(X)
+    G, C = X.shape
+    if center_val is None:
+        center_val = float(np.mean(X))
+    roff, ridx = groups_to_csr(ref_groups)
+    soff, sidx = groups_to_csr(subclusters)
+    npair = len(subclusters) * len(ref_groups)
+    Y = np.empty_like(X, order="F") if want_y else None
+    p_raw = np.empty((G, npair), dtype=np.float64, order="F")
+    p_adj = np.empty((G, npair), dtype=np.float64, order="F")
+    _lib.check(_lib.load().icnv_mask_non_de_f64(
+        _p(X), _p(Y), G, C, _p(roff), _p(ridx), len(ref_groups), _p(soff), _p(sidx), len(subclusters),
+        _code(DE_TESTS, test, "test"), float(p_val_thresh), _code(DE_RULES, rule, "rule"), float(center_val),
+        float(jitter_mean), float(jitter_sd), int(seed) & 0xFFFFFFFFFFFFFFFF, _p(p_raw) if npair else None,
+        _p(p_adj) if npair else None))
+    return Y, p_raw, p_adj
+
+
+def mask_non_de_stats() -> dict:
+    """What the last mask call did: gene tiles, genes per tile and the device time (ms) of its stages
+    (icnv_debug_mask_non_de)."""
+    out = np.zeros(7, dtype=np.float64)
+    _lib.check(_lib.load().icnv_debug_mask_non_de(_p(out)))
+    return {"tiles": int(out[0]), "genes_per_tile": int(out[1]), "gather_ms": out[2], "group_ms": out[3],
+            "pairs_ms": out[4], "bh_ms": out[5], "mask_ms": out[6]}
+
+
 # ---- CNV region calling on the state matrix (R/inferCNV_HMM.R:706-1087) ---------------------------------------
 
 def _u8(a) -> np.ndarray:

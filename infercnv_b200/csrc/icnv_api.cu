@@ -1966,3 +1966,59 @@ int icnv_debug_random_trees(double *out5) {
 }
 
 }  // extern "C"
+
+// ---- masking of non-DE genes (kernels and the device body in icnv_de.cu) ---------------------------------------------------
+// Weak references, as for the linkage: a build without icnv_de.cu reports it as unsupported.
+namespace icnv {
+int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C, const int32_t *ref_off,
+                const int32_t *ref_idx, int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub, int test,
+                double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd, unsigned long long seed,
+                double *p_raw, double *p_adj, void *stream, const char *who) __attribute__((weak));
+void de_mask_stats(double *out7) __attribute__((weak));
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_dev_mask_non_de_f64(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C,
+                             const int32_t *ref_off, const int32_t *ref_idx, int n_ref, const int32_t *sub_off,
+                             const int32_t *sub_idx, int n_sub, int test, double p_thresh, int rule, double mask_val,
+                             double jitter_mean, double jitter_sd, uint64_t seed, double *p_raw, double *p_adj, void *stream) {
+    if (!icnv::de_mask_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_mask_non_de_f64: this build has no DE kernels");
+    return icnv::de_mask_dev(X, ldx, Y, ldy, G, C, ref_off, ref_idx, n_ref, sub_off, sub_idx, n_sub, test, p_thresh, rule,
+                             mask_val, jitter_mean, jitter_sd, seed, p_raw, p_adj, stream, "icnv_dev_mask_non_de_f64");
+}
+
+int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *ref_off, const int32_t *ref_idx,
+                         int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub, int test, double p_thresh,
+                         int rule, double mask_val, double jitter_mean, double jitter_sd, uint64_t seed, double *p_raw,
+                         double *p_adj) {
+    if (!icnv::de_mask_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_mask_non_de_f64: this build has no DE kernels");
+    ICNV_HOST_PROLOGUE();
+    if (!X || G <= 0 || C <= 0 || n_ref < 1 || n_sub < 0) return set_error(ICNV_E_BAD_ARG, "icnv_mask_non_de_f64: bad argument");
+    const int64_t npair = (int64_t)n_sub * n_ref;
+    int rc;
+    double *dX = nullptr;
+    double *d_p = (p_raw || p_adj) && npair > 0 ? (double *)scratch(SLOT_OUT, sizeof(double) * 2 * (size_t)(G * npair)) : nullptr;
+    if ((p_raw || p_adj) && npair > 0 && !d_p) return ICNV_E_NOMEM;
+    if ((rc = upload_matrix(X, G * C, &dX, SLOT_IN, st))) return rc;
+    // the mask is written in place over the device copy (each entry is read and written by the same thread)
+    if ((rc = icnv::de_mask_dev(dX, G, Y ? dX : nullptr, G, G, C, ref_off, ref_idx, n_ref, sub_off, sub_idx, n_sub, test,
+                                p_thresh, rule, mask_val, jitter_mean, jitter_sd, seed, d_p, d_p ? d_p + G * npair : nullptr,
+                                st, "icnv_mask_non_de_f64")))
+        return rc;
+    if (Y) ICNV_CUDA(cudaMemcpyAsync(Y, dX, sizeof(double) * (size_t)(G * C), cudaMemcpyDeviceToHost, st));
+    if (p_raw && d_p) ICNV_CUDA(cudaMemcpyAsync(p_raw, d_p, sizeof(double) * (size_t)(G * npair), cudaMemcpyDeviceToHost, st));
+    if (p_adj && d_p)
+        ICNV_CUDA(cudaMemcpyAsync(p_adj, d_p + G * npair, sizeof(double) * (size_t)(G * npair), cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return ICNV_OK;
+}
+
+int icnv_debug_mask_non_de(double *out7) {
+    if (!out7) return set_error(ICNV_E_BAD_ARG, "icnv_debug_mask_non_de: out7 is NULL");
+    for (int i = 0; i < 7; ++i) out7[i] = 0.0;
+    if (icnv::de_mask_stats) icnv::de_mask_stats(out7);
+    return ICNV_OK;
+}
+
+}  // extern "C"

@@ -446,6 +446,31 @@ class Engine:
         m = merge.cpu().numpy().T
         return m, height.cpu().numpy(), hclust_order(m), perm_max.cpu().numpy()
 
+    def mask_non_de(self, X, ref_groups, subclusters, test="wilcoxon", p_val_thresh=0.05, rule="any", center_val=None,
+                    jitter_mean=1e-4, jitter_sd=1e-4, seed=0, out=None):
+        """mask_non_DE_genes_basic on the resident (C, G) float64 tensor X (single GPU), as api.mask_non_de_genes: returns
+        device tensors (Y, p_raw, p_adj), Y (C, G) like X (`out`, which may be X itself, or a new tensor), p_raw / p_adj
+        (n_pairs, G), row s * n_ref + j.  center_val defaults to the mean of X."""
+        from .api import DE_RULES, DE_TESTS, _code
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X.shape
+        if center_val is None:
+            center_val = float(X.mean())
+        roff, ridx = groups_to_csr(ref_groups)
+        soff, sidx = groups_to_csr(subclusters)
+        npair = len(subclusters) * len(ref_groups)
+        Y = torch.empty_like(X) if out is None else out
+        p_raw = torch.empty((npair, G), dtype=torch.float64, device=self.tdev)
+        p_adj = torch.empty((npair, G), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_mask_non_de_f64(
+            X.data_ptr(), max(X.stride(0), G), Y.data_ptr(), max(Y.stride(0), G), G, C, roff.ctypes.data, ridx.ctypes.data,
+            len(ref_groups), soff.ctypes.data, sidx.ctypes.data, len(subclusters), _code(DE_TESTS, test, "test"),
+            float(p_val_thresh), _code(DE_RULES, rule, "rule"), float(center_val), float(jitter_mean), float(jitter_sd),
+            int(seed) & 0xFFFFFFFFFFFFFFFF, p_raw.data_ptr() if npair else None, p_adj.data_ptr() if npair else None,
+            _stream_ptr()))
+        return Y, p_raw, p_adj
+
     def mean_sd(self, X, groups_local):
         """mu / sigma over all values of the listed cells across ALL ranks (.i3HMM_get_sd_trend_by_num_cells_fit,
         R/inferCNV_i3HMM.R:17-30).  groups_local: per group, this rank's LOCAL columns (the planner's slices).

@@ -565,6 +565,60 @@ b200_.parameterize_random_cluster_heights_smoothed_trees <- function(expr_matrix
     orig(expr_matrix, hclust_method, window_size, plot)
 }
 
+## mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52), run()'s step 21: every (subcluster, reference group) test,
+## BH and the mask in one GPU call, with the original's two messages per pair.  The Wilcoxon jitter comes from the
+## library's generator (rnorm's law, mean 1e-4, sd 1e-4), seeded by two draws of R's RNG; reference-side draws are shared by
+## all subclusters (INTEGRATION.md section 4).  Falls back for test.use = "perm", a non-double or NA-holding matrix, NULL or
+## duplicated rownames, duplicated pair names, an unknown require_DE_all_normals (the original's stop()), or a library error.
+b200_mask_non_DE_genes_basic <- function(infercnv_obj, p_val_thresh = 0.05, test.use = "wilcoxon",
+                                         center_val = mean(infercnv_obj@expr.data), require_DE_all_normals = "any") {
+    orig <- .icnv_env$orig$mask_non_DE_genes_basic
+    m <- infercnv_obj@expr.data
+    rules <- c(any = 0L, most = 1L, all = 2L)
+    tests <- c(wilcoxon = 0L, t = 1L)
+    refs <- infercnv_obj@reference_grouped_cell_indices
+    ok <- .icnv_enabled() && is.matrix(m) && is.double(m) && !anyNA(m) && !is.null(rownames(m)) &&
+        !anyDuplicated(rownames(m)) && is.character(test.use) && length(test.use) == 1 && test.use %in% names(tests) &&
+        is.character(require_DE_all_normals) && length(require_DE_all_normals) == 1 &&
+        require_DE_all_normals %in% names(rules) && length(refs) > 0 && is.numeric(center_val) && length(center_val) == 1
+    if (ok) {
+        ## get_DE_genes_basic's loop (:213-224): a group whose subclusters are not a (named) list is tested for nothing
+        sub_names <- character(0)
+        subs <- list()
+        for (tumor_type in names(infercnv_obj@observation_grouped_cell_indices)) {
+            indices <- infercnv_obj@tumor_subclusters[["subclusters"]][[tumor_type]]
+            if (is.list(indices)) for (nm in names(indices)) {
+                sub_names <- c(sub_names, nm)
+                subs[[length(subs) + 1]] <- as.integer(indices[[nm]])
+            }
+        }
+        pairs <- as.vector(t(outer(sub_names, names(refs), paste, sep = ",")))
+        ok <- !anyDuplicated(pairs)
+    }
+    if (ok) {
+        seed <- as.double(c(sample.int(2^31 - 1, 1), sample.int(2^31 - 1, 1)))
+        res <- .icnv_try(.Call("icnvR_mask_non_de", m, lapply(refs, as.integer), subs, tests[[test.use]],
+                               as.double(p_val_thresh), rules[[require_DE_all_normals]], as.double(center_val), seed),
+                         "mask_non_DE_genes_basic")
+        if (!is.null(res)) {
+            p_adj <- res[[2]]
+            k <- 0L
+            for (s in seq_along(subs)) for (normal_type in names(refs)) {
+                k <- k + 1L
+                futile.logger::flog.info(sprintf("Finding DE genes between %s and %s", sub_names[[s]], normal_type))
+                p <- p_adj[, k]
+                futile.logger::flog.info(sprintf("Found %d genes / %d total as DE", sum(p < p_val_thresh, na.rm = TRUE) +
+                                                 sum(is.na(p)), length(p)))
+            }
+            dimnames(res[[1]]) <- dimnames(m)
+            infercnv_obj@expr.data <- res[[1]]
+            return(infercnv_obj)
+        }
+    }
+    orig(infercnv_obj, p_val_thresh = p_val_thresh, test.use = test.use, center_val = center_val,
+         require_DE_all_normals = require_DE_all_normals)
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -573,6 +627,7 @@ infercnvb200_install <- function() {
              "get_predicted_CNV_regions", "remove_outliers_norm", "clear_noise",
              "predict_CNV_via_HMM_on_tumor_subclusters_per_chr", "i3HMM_predict_CNV_via_HMM_on_tumor_subclusters",
              "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
+             "mask_non_DE_genes_basic",
              ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
              ".parameterize_random_cluster_heights_smoothed_trees")
     ns <- asNamespace("infercnv")

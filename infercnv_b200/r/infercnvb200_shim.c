@@ -483,6 +483,32 @@ SEXP icnvR_scale(SEXP expr) {
     return ans;
 }
 
+/* mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52): the masked matrix and p_adj (G x n_sub n_ref) of the tested
+ * subclusters (lists of 1-based columns, R's loop order) against the reference groups.  test 0 wilcoxon / 1 t, rule
+ * 0 any / 1 most / 2 all; seed: two whole numbers in [0, 2^31) drawn from R's RNG, combined as hi * 2^32 + lo. */
+SEXP icnvR_mask_non_de(SEXP expr, SEXP ref_groups, SEXP subclusters, SEXP test, SEXP p_thresh, SEXP rule, SEXP center_val,
+                       SEXP seed) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    if (Rf_length(seed) != 2) Rf_error("infercnv_b200: the mask needs two seeds");
+    uint64_t sd = ((uint64_t)REAL(seed)[0] << 32) | (uint64_t)REAL(seed)[1];
+    int32_t *roff = NULL, *ridx = NULL, *soff = NULL, *sidx = NULL;
+    int n_ref = list_to_csr(ref_groups, &roff, &ridx), n_sub = list_to_csr(subclusters, &soff, &sidx);
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 2));
+    SEXP y = Rf_allocMatrix(REALSXP, (int)G, (int)C);
+    SET_VECTOR_ELT(ans, 0, y);
+    SEXP padj = Rf_allocMatrix(REALSXP, (int)G, n_sub > 0 && n_ref > 0 ? n_sub * n_ref : 0);
+    SET_VECTOR_ELT(ans, 1, padj);
+    int rc = (n_ref < 0 || n_sub < 0) ? ICNV_E_NOMEM
+             : icnv_mask_non_de_f64(REAL(expr), REAL(y), G, C, roff, ridx, n_ref, soff, sidx, n_sub, Rf_asInteger(test),
+                                    Rf_asReal(p_thresh), Rf_asInteger(rule), Rf_asReal(center_val), 1e-4, 1e-4, sd, NULL,
+                                    n_sub > 0 ? REAL(padj) : NULL);
+    free(roff); free(ridx); free(soff); free(sidx);
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 SEXP icnvR_available(void) { return Rf_ScalarLogical(icnv_device_count() > 0 && icnv_init(-1) == 0); }
 
 static const R_CallMethodDef call_methods[] = {
@@ -500,6 +526,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_knn", (DL_FUNC)&icnvR_knn, 2},
     {"icnvR_runmean", (DL_FUNC)&icnvR_runmean, 4},
     {"icnvR_random_tree_heights", (DL_FUNC)&icnvR_random_tree_heights, 5},
+    {"icnvR_mask_non_de", (DL_FUNC)&icnvR_mask_non_de, 8},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -703,3 +703,57 @@ def parameterize_random_cluster_heights_smoothed_trees(expr_matrix, hclust_metho
     h_obs = {"merge": merge, "height": height, "order": order, "labels": None, "method": hclust_method,
              "dist.method": "euclidean"}
     return {"h_obs": h_obs, "max_h": float(height.max()), "rand_max_height_dist": perm_max}
+
+
+def _tested_subclusters(infercnv_obj: Infercnv):
+    """get_DE_genes_basic's loop (R/inferCNV_mask_non_DE.R:213-224): per observation group in order, its subclusters when
+    they are a named list (a dict here), nothing when they are a plain index vector (R wraps it in an unnamed list)."""
+    subs = (infercnv_obj.tumor_subclusters or {}).get("subclusters", {})
+    names, lists = [], []
+    for group in infercnv_obj.observation_grouped_cell_indices:
+        v = subs.get(group)
+        if isinstance(v, dict):
+            for name, idx in v.items():
+                names.append(name)
+                lists.append(np.asarray(idx, dtype=np.int32))
+    return names, lists
+
+
+def get_DE_genes_basic(infercnv_obj: Infercnv, p_val_thresh: float = 0.05, test_use: str = "wilcoxon", seed: int = 0) -> dict:
+    """`get_DE_genes_basic` (R/inferCNV_mask_non_DE.R:158-259): {"<subcluster>,<reference group>": {tumor_indices, normal,
+    pvals (BH-adjusted), de_genes (gene indices with pvals < p_val_thresh)}} in R's pair order, with R's two messages per
+    pair.  The Wilcoxon jitter comes from the library's generator at `seed`."""
+    refs = list(infercnv_obj.reference_grouped_cell_indices.items())
+    names, lists = _tested_subclusters(infercnv_obj)
+    _, _, p_adj = api.mask_non_de_genes(infercnv_obj.expr_data, [np.asarray(v) for _, v in refs], lists, test=test_use,
+                                        p_val_thresh=p_val_thresh, seed=seed, want_y=False)
+    out = {}
+    for s, (name, idx) in enumerate(zip(names, lists)):
+        for j, (normal, _) in enumerate(refs):
+            log.info("Finding DE genes between %s and %s", name, normal)
+            p = p_adj[:, s * len(refs) + j]
+            genes = np.flatnonzero(p < p_val_thresh)
+            log.info("Found %d genes / %d total as DE", len(genes) + int(np.isnan(p).sum()), len(p))
+            out[f"{name},{normal}"] = {"tumor_indices": idx, "normal": normal, "pvals": p, "de_genes": genes}
+    return out
+
+
+def mask_non_DE_genes_basic(infercnv_obj: Infercnv, p_val_thresh: float = 0.05, test_use: str = "wilcoxon",
+                            center_val: Optional[float] = None, require_DE_all_normals: str = "any",
+                            seed: int = 0) -> Infercnv:
+    """`mask_non_DE_genes_basic` (R/inferCNV_mask_non_DE.R:28-52): entries of genes not DE against the reference groups (by
+    require_DE_all_normals) set to center_val (default: the mean of expr.data), one GPU call (icnv_mask_non_de_f64)."""
+    if require_DE_all_normals not in api.DE_RULES:
+        raise ValueError(f"Error, not recognizing require_DE_all_normals={require_DE_all_normals}")
+    refs = [np.asarray(v) for v in infercnv_obj.reference_grouped_cell_indices.values()]
+    names, lists = _tested_subclusters(infercnv_obj)
+    Y, _, p_adj = api.mask_non_de_genes(infercnv_obj.expr_data, refs, lists, test=test_use, p_val_thresh=p_val_thresh,
+                                        rule=require_DE_all_normals, center_val=center_val, seed=seed)
+    for s, name in enumerate(names):
+        for j, normal in enumerate(infercnv_obj.reference_grouped_cell_indices):
+            p = p_adj[:, s * len(refs) + j]
+            log.info("Finding DE genes between %s and %s", name, normal)
+            log.info("Found %d genes / %d total as DE", int((p < p_val_thresh).sum() + np.isnan(p).sum()), len(p))
+    out = copy.copy(infercnv_obj)
+    out.expr_data = Y
+    return out
