@@ -341,6 +341,35 @@ ICNV_API int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t
  * (c) pair tests, (d) BH, (e) mask} (device time summed over the tiles); zeros before any call. */
 ICNV_API int icnv_debug_mask_non_de(double *out7);
 
+/* Gibbs sampling of inferCNVBayesNet (R/inferCNV_BayesNet.R run_gibb_sampling, :1054-1107; run() step 18) for n_reg CNV
+ * regions of the G x C matrix X in one call - the posterior JAGS samples, not its draws.
+ *   Regions (CSR, 0-based): genes gene_idx[gene_off[r] .. gene_off[r+1]), cells cell_idx[cell_off[r] .. cell_off[r+1]), both
+ *   non-empty.  pooled (nullable u8 per region): R's one-gene quirk - the region is ONE pseudo-cell whose "genes" are all its
+ *   entries (cells in list order, within a cell its genes in list order); C'_r = 1 for a pooled region, C_r otherwise.
+ *   Model: x ~ dnorm(mu[eps], tau[eps]) (tau a precision), eps_j ~ dcat(theta), theta ~ ddirich(1, ..., 1), m = 2..8 states.
+ *   L[j, k] = sum over the region's entries of column j of (1/2 log tau_k - 1/2 tau_k (x - mu_k)^2), FP64 in list order.
+ *   n_chains chains (chain c starts from eps = c mod m, as R's inits rep(c, C)), n_burn discarded sweeps, then n_keep kept,
+ *   thin 1; a sweep draws theta | eps ~ Dirichlet(1 + n) (Marsaglia-Tsang gammas, FP64), then eps_j | theta with weights
+ *   theta_k exp(L[j, k]): FP64 log-weights less their maximum, exp and cumulative sum in FP32 (each normalised weight within
+ *   1e-6 absolute: expf's 2 ulp, the FP32 rounding of the argument and of the sum stay under 8e-7).  Every draw is keyed
+ *   by (seed, region, chain, sweep, state or column, rejection attempt) through mix64 / hash3, so the result is a pure
+ *   function of (seed, inputs), whatever the launch shape or the thread order.
+ *   Device memory besides the outputs: L (when loglik is NULL) and one private count buffer per sampler CTA of
+ *   ceil(max_r C'_r / 256) * 256 * m int32 - (2 x SM count) CTAs, e.g. 634 MB for 264 CTAs at 100 000 cells and m = 6.
+ * theta: per region r at offset r n_chains n_keep m, a column-major (n_chains n_keep) x m block, chains stacked in order (R's
+ * do.call(rbind, chains)).  state_counts (int32) and loglik (nullable): per region an m x C'_r column-major block at offset
+ * m sum_{s<r} C'_s; state_counts[k, j] = kept draws of column j in state k over all chains (sums to n_chains n_keep).
+ * An empty gene or cell list, an index out of range, m outside 2..8, tau <= 0, a non-finite mu or tau, n_chains < 1,
+ * n_keep < 1 or n_burn < 0: ICNV_E_BAD_ARG; NaN / Inf in a listed entry: ICNV_E_NONFINITE; not enough device memory:
+ * ICNV_E_NOMEM.  Pageable X goes up through the pinned staging ring. */
+ICNV_API int icnv_bayesnet_f64(const double *X, int64_t G, int64_t C, const int32_t *gene_off, const int32_t *gene_idx,
+                               const int32_t *cell_off, const int32_t *cell_idx, const uint8_t *pooled, int n_reg, int m,
+                               const double *mu, const double *tau, int n_chains, int n_burn, int n_keep, uint64_t seed,
+                               double *theta, int32_t *state_counts, double *loglik);
+/* What the last Bayesian network call did: out4 = {regions, sampler CTAs, ms of (a) the log-likelihood pass, (b) the
+ * sampler}; zeros before any call. */
+ICNV_API int icnv_debug_bayesnet(double *out4);
+
 /* Combine per-cell (sum, sd) pairs - e.g. all-gathered from several GPUs - into mu / sigma over all values
  * of those cells, in list order (what icnv_mean_sd_f64 does internally). */
 ICNV_API void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, int64_t G, double *mu,
@@ -529,6 +558,13 @@ ICNV_API int icnv_dev_mask_non_de_f64(const double *X, int64_t ldx, double *Y, i
                                       const int32_t *sub_off /*host*/, const int32_t *sub_idx /*host*/, int n_sub, int test,
                                       double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd,
                                       uint64_t seed, double *p_raw, double *p_adj, void *stream);
+/* icnv_bayesnet_f64 on device pointers: X (column stride ldx >= G), theta, state_counts, loglik (nullable); the region lists,
+ * pooled, mu and tau are HOST arrays.  Synchronises `stream` after the log-likelihood pass (non-finite check) and at the end. */
+ICNV_API int icnv_dev_bayesnet_f64(const double *X, int64_t ldx, int64_t G, int64_t C, const int32_t *gene_off /*host*/,
+                                   const int32_t *gene_idx /*host*/, const int32_t *cell_off /*host*/,
+                                   const int32_t *cell_idx /*host*/, const uint8_t *pooled /*host*/, int n_reg, int m,
+                                   const double *mu /*host*/, const double *tau /*host*/, int n_chains, int n_burn, int n_keep,
+                                   uint64_t seed, double *theta, int32_t *state_counts, double *loglik, void *stream);
 /* Region calling on device-resident states (uint8, column stride lds >= G).
  * icnv_dev_state_counts_u8: counts[(k*G + g)*8 + slot] = number of cells of group k (d_cells[h_grp_off[k] ..
  * h_grp_off[k+1]), device) whose state at gene g falls in `slot` (0: unassigned, v+1: state v); integer counts, so

@@ -472,6 +472,62 @@ def mask_non_de_stats() -> dict:
             "pairs_ms": out[4], "bh_ms": out[5], "mask_ms": out[6]}
 
 
+def _bayesnet_args(regions_genes, regions_cells, mu, tau, pooled):
+    goff, gidx = groups_to_csr(regions_genes)
+    coff, cidx = groups_to_csr(regions_cells)
+    n_reg = len(regions_genes)
+    if len(regions_cells) != n_reg:
+        raise ValueError("regions_genes and regions_cells differ in length")
+    pool = np.zeros(max(n_reg, 1), dtype=np.uint8)
+    if pooled is not None:
+        pool[:n_reg] = np.asarray(pooled, dtype=bool)
+    mu = np.ascontiguousarray(mu, dtype=np.float64)
+    tau = np.ascontiguousarray(tau, dtype=np.float64)
+    if mu.shape != tau.shape or mu.ndim != 1:
+        raise ValueError("mu and tau must be vectors of the same length")
+    ncol = np.where(pool[:n_reg] > 0, 1, np.diff(coff)).astype(np.int64)
+    return goff, gidx, coff, cidx, pool, mu, tau, ncol
+
+
+def _bayesnet_split(theta, counts, loglik, ncol, m, rows):
+    """Flat library outputs -> per-region lists."""
+    off = np.concatenate([[0], np.cumsum(ncol)]) * m
+    th = [theta[r * rows * m:(r + 1) * rows * m].reshape((rows, m), order="F") for r in range(len(ncol))]
+    cnt = [counts[off[r]:off[r + 1]].reshape((m, int(ncol[r])), order="F") for r in range(len(ncol))]
+    ll = None if loglik is None else [loglik[off[r]:off[r + 1]].reshape((m, int(ncol[r])), order="F") for r in range(len(ncol))]
+    return {"theta": th, "cell_probabilities": [c / float(rows) for c in cnt], "state_counts": cnt, "loglik": ll}
+
+
+def bayesnet(X, regions_genes, regions_cells, mu, tau, n_chains, n_burn=700, n_keep=1000, seed=0, pooled=None,
+             want_loglik=False) -> dict:
+    """inferCNVBayesNet's Gibbs sampling (icnv_bayesnet_f64) for every region of the genes x cells matrix X: region r is
+    the block X[regions_genes[r], regions_cells[r]] (0-based lists), mu / tau the m states' means and precisions; pooled[r]
+    marks R's one-gene quirk (the region is one pseudo-cell).  Returns {"theta": per region the (n_chains n_keep) x m draws,
+    chains stacked; "cell_probabilities": per region m x C'_r state frequencies; "state_counts": the same as integer counts;
+    "loglik": per region the m x C'_r log-likelihoods L, or None}.  Same posterior as JAGS, not its draws."""
+    X = _f64(X)
+    G, C = X.shape
+    goff, gidx, coff, cidx, pool, mu, tau, ncol = _bayesnet_args(regions_genes, regions_cells, mu, tau, pooled)
+    n_reg, m = len(regions_genes), len(mu)
+    rows = int(n_chains) * int(n_keep)
+    mm = m if 2 <= m <= 8 else 2
+    theta = np.empty(max(n_reg * max(rows, 1) * mm, 1), dtype=np.float64)
+    counts = np.empty(max(int(ncol.sum()) * mm, 1), dtype=np.int32)
+    loglik = np.empty(max(int(ncol.sum()) * mm, 1), dtype=np.float64) if want_loglik else None
+    _lib.check(_lib.load().icnv_bayesnet_f64(
+        _p(X), G, C, _p(goff), _p(gidx), _p(coff), _p(cidx), _p(pool), n_reg, m, _p(mu), _p(tau), int(n_chains), int(n_burn),
+        int(n_keep), int(seed) & 0xFFFFFFFFFFFFFFFF, _p(theta), _p(counts), _p(loglik)))
+    return _bayesnet_split(theta, counts, loglik, ncol, m, rows)
+
+
+def bayesnet_stats() -> dict:
+    """What the last Bayesian network call did: regions, sampler CTAs and the device time (ms) of the log-likelihood pass
+    and of the sampler (icnv_debug_bayesnet)."""
+    out = np.zeros(4, dtype=np.float64)
+    _lib.check(_lib.load().icnv_debug_bayesnet(_p(out)))
+    return {"regions": int(out[0]), "ctas": int(out[1]), "loglik_ms": out[2], "sampler_ms": out[3]}
+
+
 # ---- CNV region calling on the state matrix (R/inferCNV_HMM.R:706-1087) ---------------------------------------
 
 def _u8(a) -> np.ndarray:

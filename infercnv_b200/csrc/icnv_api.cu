@@ -2022,3 +2022,102 @@ int icnv_debug_mask_non_de(double *out7) {
 }
 
 }  // extern "C"
+
+// ---- Bayesian network filter (kernels and the device body in icnv_bayes.cu) -------------------------------------------------
+// Weak references, as for the linkage: a build without icnv_bayes.cu reports it as unsupported.
+namespace icnv {
+int bayesnet_dev(const double *X, int64_t ldx, int64_t G, int64_t C, const int32_t *gene_off, const int32_t *gene_idx,
+                 const int32_t *cell_off, const int32_t *cell_idx, const uint8_t *pooled, int n_reg, int m, const double *mu,
+                 const double *tau, int n_chains, int n_burn, int n_keep, unsigned long long seed, double *theta,
+                 int32_t *state_counts, double *loglik, void *stream, const char *who) __attribute__((weak));
+void bayesnet_stats(double *out4) __attribute__((weak));
+int bayesnet_check(int64_t G, int64_t C, const int32_t *gene_off, const int32_t *gene_idx, const int32_t *cell_off,
+                   const int32_t *cell_idx, const uint8_t *pooled, int n_reg, int m, const double *mu, const double *tau,
+                   int n_chains, int n_burn, int n_keep, int64_t *n_cols, const char *who) __attribute__((weak));
+
+// The G x C host matrix into SLOT_IN.  Page-locked memory goes over PCIe directly; pageable memory (an R matrix) goes through
+// the two pinned ring slots in chunks, the copy threads filling one slot while the other one's DMA runs.
+static int upload_matrix_ring(const double *X, int64_t n, double **dX, cudaStream_t st) {
+    Ctx &c = ctx();
+    *dX = (double *)scratch(SLOT_IN, sizeof(double) * (size_t)n);
+    if (!*dX) return ICNV_E_NOMEM;
+    if (is_pinned(X)) {
+        ICNV_CUDA(cudaMemcpyAsync(*dX, X, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, st));
+        return ICNV_OK;
+    }
+    const int64_t chunk = std::min<int64_t>(n, (int64_t)40 << 20);   // 320 MB per ring slot
+    double *p[2];
+    for (int b = 0; b < 2; ++b)
+        if (!(p[b] = (double *)pinned(b, sizeof(double) * (size_t)chunk))) return ICNV_E_NOMEM;
+    CopyPool pool(pool_threads_per_device());
+    int64_t i = 0;
+    for (int64_t q = 0; q < n; q += chunk, ++i) {
+        const int b = (int)(i & 1);
+        const int64_t nq = std::min<int64_t>(chunk, n - q);
+        ICNV_CUDA(cudaEventSynchronize(c.ev_h2d[b]));   // the slot's previous DMA is done (a recorded-never event is complete)
+        pool.copy2(p[b], X + q, sizeof(double) * (size_t)nq, nullptr, nullptr, 0);
+        ICNV_CUDA(cudaMemcpyAsync(*dX + q, p[b], sizeof(double) * (size_t)nq, cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaEventRecord(c.ev_h2d[b], st));
+    }
+    return ICNV_OK;
+}
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_dev_bayesnet_f64(const double *X, int64_t ldx, int64_t G, int64_t C, const int32_t *gene_off, const int32_t *gene_idx,
+                          const int32_t *cell_off, const int32_t *cell_idx, const uint8_t *pooled, int n_reg, int m,
+                          const double *mu, const double *tau, int n_chains, int n_burn, int n_keep, uint64_t seed,
+                          double *theta, int32_t *state_counts, double *loglik, void *stream) {
+    if (!icnv::bayesnet_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_bayesnet_f64: this build has no Bayesian network kernels");
+    return icnv::bayesnet_dev(X, ldx, G, C, gene_off, gene_idx, cell_off, cell_idx, pooled, n_reg, m, mu, tau, n_chains, n_burn,
+                              n_keep, seed, theta, state_counts, loglik, stream, "icnv_dev_bayesnet_f64");
+}
+
+int icnv_bayesnet_f64(const double *X, int64_t G, int64_t C, const int32_t *gene_off, const int32_t *gene_idx,
+                      const int32_t *cell_off, const int32_t *cell_idx, const uint8_t *pooled, int n_reg, int m,
+                      const double *mu, const double *tau, int n_chains, int n_burn, int n_keep, uint64_t seed, double *theta,
+                      int32_t *state_counts, double *loglik) {
+    if (!icnv::bayesnet_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_bayesnet_f64: this build has no Bayesian network kernels");
+    ICNV_HOST_PROLOGUE();
+    if (!X || !theta || !state_counts) return set_error(ICNV_E_BAD_ARG, "icnv_bayesnet_f64: bad argument");
+    // every host-side check before the matrix goes up
+    int64_t n_cols = 0;
+    int rc = icnv::bayesnet_check(G, C, gene_off, gene_idx, cell_off, cell_idx, pooled, n_reg, m, mu, tau, n_chains, n_burn,
+                                  n_keep, &n_cols, "icnv_bayesnet_f64");
+    if (rc || n_reg == 0) return rc;
+    const int64_t mm = m;
+    const size_t b_theta = sizeof(double) * (size_t)n_reg * (size_t)n_chains * (size_t)n_keep * (size_t)mm,
+                 b_counts = sizeof(int32_t) * (size_t)(n_cols * mm), b_ll = loglik ? sizeof(double) * (size_t)(n_cols * mm) : 0;
+    double *dX = nullptr;
+    if ((rc = upload_matrix_ring(X, G * C, &dX, st))) return rc;
+    char *d_out = nullptr;
+    if (cudaMalloc((void **)&d_out, b_theta + b_counts + b_ll + 512) != cudaSuccess) {
+        cudaGetLastError();
+        return set_error(ICNV_E_NOMEM, "icnv_bayesnet_f64: no room for the %zu-byte theta draws", b_theta);
+    }
+    double *d_theta = (double *)d_out;
+    int32_t *d_counts = (int32_t *)(d_out + ((b_theta + 255) & ~(size_t)255));
+    double *d_ll = loglik ? (double *)(d_out + ((b_theta + 255) & ~(size_t)255) + ((b_counts + 255) & ~(size_t)255)) : nullptr;
+    rc = icnv::bayesnet_dev(dX, G, G, C, gene_off, gene_idx, cell_off, cell_idx, pooled, n_reg, m, mu, tau, n_chains, n_burn,
+                            n_keep, seed, d_theta, d_counts, d_ll, st, "icnv_bayesnet_f64");
+    if (!rc) {
+        cudaError_t e = cudaMemcpyAsync(theta, d_theta, b_theta, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(state_counts, d_counts, b_counts, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && loglik) e = cudaMemcpyAsync(loglik, d_ll, b_ll, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) rc = set_error(ICNV_E_CUDA, "icnv_bayesnet_f64: copy back failed: %s", cudaGetErrorString(e));
+    }
+    cudaStreamSynchronize(st);
+    cudaFree(d_out);
+    return rc;
+}
+
+int icnv_debug_bayesnet(double *out4) {
+    if (!out4) return set_error(ICNV_E_BAD_ARG, "icnv_debug_bayesnet: out4 is NULL");
+    for (int i = 0; i < 4; ++i) out4[i] = 0.0;
+    if (icnv::bayesnet_stats) icnv::bayesnet_stats(out4);
+    return ICNV_OK;
+}
+
+}  // extern "C"

@@ -170,6 +170,13 @@ __device__ __forceinline__ uint64_t mix64(uint64_t z) {  // splitmix64 finaliser
 __device__ __forceinline__ uint64_t hash3(uint64_t seed, uint64_t a, uint64_t b, uint64_t c) {
     return mix64(mix64(mix64(seed ^ 0x243f6a8885a308d3ull) + a) * 0x9fb21c651e98df25ull + b) ^ mix64(c + 0x13198a2e03707344ull);
 }
+// a (0, 1] uniform and a Box-Muller standard normal from generator words (the synthetic workload, the Gibbs sampler)
+__device__ __forceinline__ double u01(uint64_t h) {  // (0, 1]
+    return ((double)(h >> 11) + 1.0) * (1.0 / 9007199254740992.0);
+}
+__device__ __forceinline__ double std_normal(uint64_t h1, uint64_t h2) {
+    return sqrt(-2.0 * log(u01(h1))) * cospi(2.0 * u01(h2));
+}
 __device__ __forceinline__ double warp_min_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));

@@ -13,13 +13,6 @@
 
 namespace icnv {
 
-__device__ __forceinline__ double u01(uint64_t h) {  // (0, 1]
-    return ((double)(h >> 11) + 1.0) * (1.0 / 9007199254740992.0);
-}
-__device__ __forceinline__ double std_normal(uint64_t h1, uint64_t h2) {
-    return sqrt(-2.0 * log(u01(h1))) * cospi(2.0 * u01(h2));
-}
-
 __global__ void __launch_bounds__(256) synth_kernel(double *__restrict__ X, int64_t G, int64_t cell0, int64_t n_cells,
                                                     int64_t C_total, const int32_t *__restrict__ chr_of, int K,
                                                     uint64_t seed) {

@@ -471,6 +471,29 @@ class Engine:
             _stream_ptr()))
         return Y, p_raw, p_adj
 
+    def bayesnet(self, X, regions_genes, regions_cells, mu, tau, n_chains, n_burn=700, n_keep=1000, seed=0, pooled=None,
+                 want_loglik=False) -> dict:
+        """inferCNVBayesNet's Gibbs sampling on the resident (C, G) float64 tensor X (single GPU), as api.bayesnet and
+        bit-identical to it; the outputs come back to the host as the same per-region lists."""
+        from .api import _bayesnet_args, _bayesnet_split
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X.shape
+        goff, gidx, coff, cidx, pool, mu, tau, ncol = _bayesnet_args(regions_genes, regions_cells, mu, tau, pooled)
+        n_reg, m = len(regions_genes), len(mu)
+        rows = int(n_chains) * int(n_keep)
+        mm = m if 2 <= m <= 8 else 2
+        theta = torch.empty(max(n_reg * max(rows, 1) * mm, 1), dtype=torch.float64, device=self.tdev)
+        counts = torch.empty(max(int(ncol.sum()) * mm, 1), dtype=torch.int32, device=self.tdev)
+        loglik = torch.empty(max(int(ncol.sum()) * mm, 1), dtype=torch.float64, device=self.tdev) if want_loglik else None
+        _lib.check(self.lib.icnv_dev_bayesnet_f64(
+            X.data_ptr(), max(X.stride(0), G), G, C, goff.ctypes.data, gidx.ctypes.data, coff.ctypes.data, cidx.ctypes.data,
+            pool.ctypes.data, n_reg, m, mu.ctypes.data, tau.ctypes.data, int(n_chains), int(n_burn), int(n_keep),
+            int(seed) & 0xFFFFFFFFFFFFFFFF, theta.data_ptr(), counts.data_ptr(),
+            loglik.data_ptr() if loglik is not None else None, _stream_ptr()))
+        return _bayesnet_split(theta.cpu().numpy(), counts.cpu().numpy(), None if loglik is None else loglik.cpu().numpy(),
+                               ncol, m, rows)
+
     def mean_sd(self, X, groups_local):
         """mu / sigma over all values of the listed cells across ALL ranks (.i3HMM_get_sd_trend_by_num_cells_fit,
         R/inferCNV_i3HMM.R:17-30).  groups_local: per group, this rank's LOCAL columns (the planner's slices).

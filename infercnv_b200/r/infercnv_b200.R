@@ -619,6 +619,132 @@ b200_mask_non_DE_genes_basic <- function(infercnv_obj, p_val_thresh = 0.05, test
          require_DE_all_normals = require_DE_all_normals)
 }
 
+## inferCNVBayesNet (R/inferCNV_BayesNet.R:1237-1364; run() step 18) with every region's Gibbs sampling in one library call
+## (icnv_bayesnet_f64) in place of runMCMC's one JAGS model per region: the same posterior, not JAGS's draws.  The chains
+## (6 for i6, 3 for i3, chain c from state c), 500 + 200 discarded and 1000 kept sweeps, and the outputs' shapes and dimnames
+## are the original's; a region of one gene and several cells is JAGS's single pseudo-cell (INTEGRATION.md section 4).  The
+## generator is seeded by two draws of R's RNG.  The whole original runs for diagnostics = TRUE when no_plot does not turn
+## them off (coda needs the raw chains), a model file that is not the bundled one, or a non-double or NA-holding matrix -
+## all decided before anything is logged; the original's runMCMC runs on the initialised object, with R's RNG stream as it
+## was, for a region without cells or a library error.
+b200_inferCNVBayesNet <- function( file_dir,
+                              infercnv_obj,
+                              HMM_states,
+                              out_dir,
+                              resume_file_token,
+                              model_file        = NULL,
+                              CORES             = 1,
+                              postMcmcMethod    = NULL,
+                              plotingProbs      = TRUE,
+                              quietly           = TRUE,
+                              diagnostics       = FALSE,
+                              HMM_type          = HMM_type,
+                              k_obs_groups      = k_obs_groups,
+                              cluster_by_groups = cluster_by_groups,
+                              reassignCNVs      = TRUE,
+                              no_plot           = no_plot,
+                              useRaster) {
+    orig <- .icnv_env$orig$inferCNVBayesNet
+    fallback <- function() orig(file_dir = file_dir, infercnv_obj = infercnv_obj, HMM_states = HMM_states, out_dir = out_dir,
+                                resume_file_token = resume_file_token, model_file = model_file, CORES = CORES,
+                                postMcmcMethod = postMcmcMethod, plotingProbs = plotingProbs, quietly = quietly,
+                                diagnostics = diagnostics, HMM_type = HMM_type, k_obs_groups = k_obs_groups,
+                                cluster_by_groups = cluster_by_groups, reassignCNVs = reassignCNVs, no_plot = no_plot,
+                                useRaster = useRaster)
+    bundled <- ifelse(HMM_type == "i6", system.file("BUGS_Mixture_Model", package = "infercnv"),
+                      system.file("BUGS_Mixture_Model_i3", package = "infercnv"))
+    ## no_plot overrides the plotting options first, as in the original
+    diag_on <- if (no_plot == TRUE) FALSE else isTRUE(diagnostics)
+    x <- infercnv_obj@expr.data
+    if (!.icnv_enabled() || diag_on || !is.matrix(x) || !is.double(x) || anyNA(x) ||
+        (!is.null(model_file) && !identical(normalizePath(model_file, mustWork = FALSE), normalizePath(bundled, mustWork = FALSE))))
+        return(fallback())
+    ## the original's input checks
+    if (!is.null(model_file) && !file.exists(model_file)){
+        error_message <- paste("Cannot find the model file.",
+                               "Please supply the correct path for the model file.")
+        futile.logger::flog.error(error_message)
+        stop(error_message)
+    }
+    if (!(CORES == 1)){
+        if (is.na(parallel::detectCores())){
+            futile.logger::flog.warn(paste("Unable to detect number of cores available through parallel:detectCores(), using the provided number", CORES))
+        } else if (as.integer(CORES) > parallel::detectCores()){
+            error_message <- paste("Too many cores previded. The following system has ", parallel::detectCores(), " cores.",
+                                   "Please select an appropriate amount.")
+            futile.logger::flog.error(error_message)
+            stop(error_message)
+        }
+    }
+    if(out_dir != "." & !file.exists(out_dir)){
+        dir.create(file.path(out_dir))
+        futile.logger::flog.info(paste("Creating the following Directory: ", out_dir))
+    }
+    if (is.null(model_file)) model_file <- bundled
+    if (no_plot == TRUE) {
+        plotingProbs <- FALSE
+        diagnostics <- FALSE
+    }
+    args_parsed <- list("file_dir" = file_dir, "model_file" = model_file, "CORES" = CORES, "out_dir"= out_dir,
+                        "resume_file_token" = resume_file_token, "plotingProbs" = plotingProbs,
+                        "postMcmcMethod"= postMcmcMethod, "quietly" = quietly, "BayesMaxPNormal" = 0, "HMM_type" = HMM_type,
+                        "k_obs_groups" = k_obs_groups, "cluster_by_groups" = cluster_by_groups,
+                        "reassignCNVs" = reassignCNVs, "diagnostics" = diagnostics)
+    obj <- methods::new("MCMC_inferCNV")
+    obj <- infercnv:::initializeObject(obj, args_parsed, infercnv_obj)
+    obj <- infercnv:::MeanSD(obj = obj, HMM_states = HMM_states, infercnv_obj = infercnv_obj)
+    m <- obj@expr.data
+    cg <- obj@cell_gene
+    n_states <- ifelse(HMM_type == "i6", 6L, 3L)
+    n_chains <- n_states
+    start_time <- Sys.time()
+    res <- NULL
+    if (length(cg) > 0 && !any(vapply(cg, function(i) length(i$Cells) == 0 || length(i$Genes) == 0, logical(1)))) {
+        ## the seeds are the last thing drawn before the call; a library error puts R's RNG stream back
+        had_seed <- exists(".Random.seed", envir = globalenv(), inherits = FALSE)
+        old_seed <- if (had_seed) get(".Random.seed", envir = globalenv(), inherits = FALSE) else NULL
+        seed <- as.double(c(sample.int(2^31 - 1, 1), sample.int(2^31 - 1, 1)))
+        genes <- lapply(cg, function(i) as.integer(if (is.character(i$Genes)) match(i$Genes, rownames(m)) else i$Genes))
+        cells <- lapply(cg, function(i) as.integer(if (is.character(i$Cells)) match(i$Cells, colnames(m)) else i$Cells))
+        pooled <- vapply(cg, function(i) length(i$Genes) == 1 && length(i$Cells) > 1, logical(1))
+        res <- .icnv_try(.Call("icnvR_bayesnet", m, genes, cells, as.integer(pooled), as.double(obj@mu), as.double(obj@sig),
+                               n_chains, 700L, 1000L, seed), "inferCNVBayesNet")
+        if (is.null(res)) {
+            if (had_seed) assign(".Random.seed", old_seed, envir = globalenv())
+            else if (exists(".Random.seed", envir = globalenv(), inherits = FALSE)) rm(".Random.seed", envir = globalenv())
+        }
+    }
+    if (is.null(res)) {
+        ## the original's own sampling on the object it would have built
+        obj <- infercnv:::runMCMC(obj, diagnostics)
+        res <- list(NULL, NULL)
+    }
+    if (!is.null(res[[1]])) {
+        obj@cnv_probabilities <- lapply(res[[1]], function(th) {
+            colnames(th) <- sprintf("theta[%d]", seq_len(n_states))
+            th
+        })
+        ## cell_prob's names: one epsilon column drops to a vector, which as.data.frame names "epsilons"
+        obj@cell_probabilities <- lapply(res[[2]], function(p) {
+            dimnames(p) <- list(as.character(seq_len(n_states)),
+                                if (ncol(p) == 1) "epsilons" else sprintf("epsilon[%d]", seq_len(ncol(p))))
+            p
+        })
+    }
+    end_time <- Sys.time()
+    futile.logger::flog.info(paste("Gibbs sampling time: ", difftime(end_time, start_time, units = "min")[[1]], " Minutes"))
+    saveRDS(obj, file = file.path(obj@args$out_dir, "MCMC_inferCNV_obj.rds"))
+    if (obj@args$postMcmcMethod == "removeCNV" || obj@args$reassignCNVs == TRUE ){
+        title <- sprintf(" (1 - Probabilities of Normal) Before Filtering")
+        output_filename <- "infercnv.NormalProbabilities.PreFiltering"
+    } else {
+        title <- sprintf(" 1 - Probabilities of Normal ")
+        output_filename <- "infercnv.NormalProbabilities"
+    }
+    infercnv:::postProbNormal(obj, PNormal = NULL, title = title, output_filename = output_filename, useRaster = useRaster)
+    obj
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -627,7 +753,7 @@ infercnvb200_install <- function() {
              "get_predicted_CNV_regions", "remove_outliers_norm", "clear_noise",
              "predict_CNV_via_HMM_on_tumor_subclusters_per_chr", "i3HMM_predict_CNV_via_HMM_on_tumor_subclusters",
              "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
-             "mask_non_DE_genes_basic",
+             "mask_non_DE_genes_basic", "inferCNVBayesNet",
              ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
              ".parameterize_random_cluster_heights_smoothed_trees")
     ns <- asNamespace("infercnv")

@@ -14,6 +14,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "infercnv_b200.h"
 
@@ -509,6 +510,58 @@ SEXP icnvR_mask_non_de(SEXP expr, SEXP ref_groups, SEXP subclusters, SEXP test, 
     return ans;
 }
 
+/* inferCNVBayesNet's sampling: list(theta per region ((chains x n_keep) x m), cell frequencies per region (m x C')) */
+SEXP icnvR_bayesnet(SEXP expr, SEXP genes, SEXP cells, SEXP pooled, SEXP mu, SEXP tau, SEXP n_chains, SEXP n_burn, SEXP n_keep,
+                    SEXP seed) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    if (Rf_length(seed) != 2) Rf_error("infercnv_b200: the Bayesian network needs two seeds");
+    uint64_t sd = ((uint64_t)REAL(seed)[0] << 32) | (uint64_t)REAL(seed)[1];
+    int32_t *goff = NULL, *gidx = NULL, *coff = NULL, *cidx = NULL;
+    int n_reg = list_to_csr(genes, &goff, &gidx), n_reg2 = list_to_csr(cells, &coff, &cidx);
+    int m = Rf_length(mu), nc = Rf_asInteger(n_chains), nb = Rf_asInteger(n_burn), nk = Rf_asInteger(n_keep);
+    int rc = ICNV_OK;
+    if (n_reg < 0 || n_reg2 < 0) rc = ICNV_E_NOMEM;
+    else if (n_reg != n_reg2 || Rf_length(pooled) != n_reg || Rf_length(tau) != m || m < 2 || m > 8 || nc < 1 || nk < 1)
+        rc = ICNV_E_BAD_ARG;
+    int64_t n_cols = 0;
+    uint8_t *pool = (uint8_t *)calloc((size_t)(n_reg > 0 ? n_reg : 1), 1);
+    if (!pool && rc == ICNV_OK) rc = ICNV_E_NOMEM;
+    for (int r = 0; rc == ICNV_OK && r < n_reg; ++r) {
+        pool[r] = (uint8_t)(INTEGER(pooled)[r] == 1);
+        n_cols += pool[r] ? 1 : coff[r + 1] - coff[r];
+    }
+    const int64_t rows = (int64_t)nc * nk;
+    double *theta = rc == ICNV_OK ? (double *)malloc(sizeof(double) * (size_t)(n_reg * rows * m + 1)) : NULL;
+    int32_t *counts = rc == ICNV_OK ? (int32_t *)malloc(sizeof(int32_t) * (size_t)(n_cols * m + 1)) : NULL;
+    if (rc == ICNV_OK && (!theta || !counts)) rc = ICNV_E_NOMEM;
+    if (rc == ICNV_OK)
+        rc = icnv_bayesnet_f64(REAL(expr), G, C, goff, gidx, coff, cidx, pool, n_reg, m, REAL(mu), REAL(tau), nc, nb, nk, sd,
+                               theta, counts, NULL);
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 2));
+    if (rc == ICNV_OK) {
+        SEXP th_l = Rf_allocVector(VECSXP, n_reg);
+        SET_VECTOR_ELT(ans, 0, th_l);
+        SEXP cp_l = Rf_allocVector(VECSXP, n_reg);
+        SET_VECTOR_ELT(ans, 1, cp_l);
+        int64_t off = 0;
+        for (int r = 0; r < n_reg; ++r) {
+            SEXP th = Rf_allocMatrix(REALSXP, (int)rows, m);
+            SET_VECTOR_ELT(th_l, r, th);
+            memcpy(REAL(th), theta + (int64_t)r * rows * m, sizeof(double) * (size_t)(rows * m));
+            const int ncr = pool[r] ? 1 : coff[r + 1] - coff[r];
+            SEXP cp = Rf_allocMatrix(REALSXP, m, ncr);
+            SET_VECTOR_ELT(cp_l, r, cp);
+            for (int64_t i = 0; i < (int64_t)ncr * m; ++i) REAL(cp)[i] = (double)counts[off * m + i] / (double)rows;
+            off += ncr;
+        }
+    }
+    free(goff); free(gidx); free(coff); free(cidx); free(pool); free(theta); free(counts);
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 SEXP icnvR_available(void) { return Rf_ScalarLogical(icnv_device_count() > 0 && icnv_init(-1) == 0); }
 
 static const R_CallMethodDef call_methods[] = {
@@ -527,6 +580,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_runmean", (DL_FUNC)&icnvR_runmean, 4},
     {"icnvR_random_tree_heights", (DL_FUNC)&icnvR_random_tree_heights, 5},
     {"icnvR_mask_non_de", (DL_FUNC)&icnvR_mask_non_de, 8},
+    {"icnvR_bayesnet", (DL_FUNC)&icnvR_bayesnet, 10},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -757,3 +757,84 @@ def mask_non_DE_genes_basic(infercnv_obj: Infercnv, p_val_thresh: float = 0.05, 
     out = copy.copy(infercnv_obj)
     out.expr_data = Y
     return out
+
+
+def cell_gene_from_regions(regions: list, cell_names=None, HMM_type: str = "i6") -> list:
+    """inferCNVBayesNet's @cell_gene (initializeObject / getGenesCells, R/inferCNV_BayesNet.R:245-339) from
+    get_predicted_CNV_regions' report, as R reads it back from the step-17 files: the per-gene file is written with
+    ignore_neutral_state (R/inferCNV_ops.R:1316), so regions in the neutral state (3 for i6, 2 for i3) are not there; the
+    remaining regions in file order, group by group.  Per region {"cnv_regions": name, "Genes": 0-based rows of the
+    region's genes in ascending order (which(rownames %in% genes)), "Cells": 0-based columns whose name is one of the
+    group's cells, ascending (which(colnames %in% cells)), "State": the HMM state}.  Without cell_names the report's cell
+    labels are the column indices."""
+    if HMM_type not in ("i6", "i3"):
+        raise ValueError("HMM_type must be 'i6' or 'i3'")
+    neutral = 3 if HMM_type == "i6" else 2
+    out = []
+    for grp in regions:
+        if cell_names is not None:
+            cells = np.flatnonzero(np.isin(np.asarray(cell_names, dtype=object), np.asarray(list(grp["cells"]), dtype=object)))
+        else:
+            cells = np.unique(np.asarray([int(c) for c in grp["cells"]], dtype=np.int64))
+        cells = cells.astype(np.int32)
+        cr, gr = grp["cnv_ranges"], grp["gene_regions"]
+        for i, name in enumerate(cr["cnv_name"]):
+            if int(cr["state"][i]) == neutral:
+                continue
+            out.append({"cnv_regions": name, "Genes": np.arange(gr["first_gene"][i], gr["last_gene"][i] + 1, dtype=np.int32),
+                        "Cells": cells, "State": int(cr["state"][i])})
+    return out
+
+
+def inferCNVBayesNet_sampling(expr_data, cell_gene: list, mu, sig, HMM_type: str = "i6", n_burn: int = 700,
+                              n_keep: int = 1000, seed: int = 0) -> dict:
+    """run_gibb_sampling for every region of `cell_gene` and getProbabilities (R/inferCNV_BayesNet.R:362-388, 1054-1107) in
+    one GPU call (icnv_bayesnet_f64): {"cell_gene", "cnv_probabilities": per region the (chains x 1000) x m theta draws,
+    "cell_probabilities": per region m x C' state frequencies, "HMM_type"}.  6 chains for i6, 3 for i3, chain c starting
+    from state c; a region of one gene and several cells is R's single pseudo-cell.  Same posterior as JAGS, not its
+    draws: they come from the library's generator at `seed`."""
+    if HMM_type not in ("i6", "i3"):
+        raise ValueError("HMM_type must be 'i6' or 'i3'")
+    n_chains = 6 if HMM_type == "i6" else 3
+    pooled = [len(r["Genes"]) == 1 and len(r["Cells"]) > 1 for r in cell_gene]
+    res = api.bayesnet(expr_data, [r["Genes"] for r in cell_gene], [r["Cells"] for r in cell_gene], mu, sig, n_chains,
+                       n_burn=n_burn, n_keep=n_keep, seed=seed, pooled=pooled)
+    return {"cell_gene": list(cell_gene), "cnv_probabilities": res["theta"], "cell_probabilities": res["cell_probabilities"],
+            "HMM_type": HMM_type}
+
+
+def removeCNV(mcmc: dict, HMM_states: np.ndarray, BayesMaxPNormal: float):
+    """removeCNV (R/inferCNV_BayesNet.R:562-629): every region whose mean theta of the normal state (3 for i6, 2 for i3)
+    exceeds BayesMaxPNormal is set to the normal state over its genes x cells and dropped.  Returns (mcmc, HMM_states)."""
+    normal = 3 if mcmc["HMM_type"] == "i6" else 2
+    means = [np.asarray(t).mean(axis=0) for t in mcmc["cnv_probabilities"]]
+    remove = [i for i, mt in enumerate(means) if mt[normal - 1] > BayesMaxPNormal]
+    log.info("Attempting to removing CNV(s) with a probability of being normal above  %s", BayesMaxPNormal)
+    log.info("Removing  %d  CNV(s) identified by the HMM.", len(remove))
+    if not remove:
+        return mcmc, HMM_states
+    S = HMM_states.copy()
+    for i in remove:
+        cg = mcmc["cell_gene"][i]
+        S[np.ix_(cg["Genes"], cg["Cells"])] = normal
+    keep = [i for i in range(len(means)) if i not in set(remove)]
+    out = dict(mcmc)
+    for k in ("cell_gene", "cnv_probabilities", "cell_probabilities"):
+        out[k] = [mcmc[k][i] for i in keep]
+    log.info("Total CNV's after removing:  %d", len(out["cell_gene"]))
+    return out, S
+
+
+def reassignCNV(mcmc: dict, HMM_states: np.ndarray):
+    """reassignCNV (R/inferCNV_BayesNet.R:491-539): each region's state becomes the first arg-max of its mean theta,
+    written over its genes x cells.  Returns (mcmc, HMM_states)."""
+    log.info("Reassigning CNVs based on state probabilities.")
+    S = HMM_states.copy()
+    out = dict(mcmc)
+    out["cell_gene"] = []
+    for cg, th in zip(mcmc["cell_gene"], mcmc["cnv_probabilities"]):
+        mt = np.asarray(th).mean(axis=0)
+        state = int(np.flatnonzero(mt == mt.max())[0]) + 1
+        S[np.ix_(cg["Genes"], cg["Cells"])] = state
+        out["cell_gene"].append(dict(cg, State=state))
+    return out, S
