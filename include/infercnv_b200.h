@@ -370,6 +370,33 @@ ICNV_API int icnv_bayesnet_f64(const double *X, int64_t G, int64_t C, const int3
  * sampler}; zeros before any call. */
 ICNV_API int icnv_debug_bayesnet(double *out4);
 
+/* smooth_by_chromosome_coordinates (R/inferCNV_ops.R:2534-2622; run() step 10, smooth_method = "coordinates") on the G x C
+ * matrix X, the K ranges (chr_start, chr_len) as its chromosomes.  For gene i of a range of n >= 2 genes with starts s and
+ * stops e (gene_start / gene_stop, indexed by row of X) and W = window_length >= 2:
+ *   pos = (s[i] + e[i]) / 2, around = {j : s[j] > pos - W and e[j] < pos + W} ({i} if empty; need not be contiguous),
+ *   w_j = 1 - |(e[j] + s[j]) / 2 - pos| / W, to_add = floor(|around| / 2), lo = max(0, min(around) - to_add),
+ *   hi = min(n - 1, max(around) + to_add), wv = (0.1 x (min(around) - lo), w_around, 0.1 x (hi - max(around))),
+ *   Y[i] = sum_k X[lo + k] wv[k mod |wv|] / sum(wv),  k = 0 .. hi - lo   (R's recycling where `around` has holes).
+ * W < 2, ranges of one gene and the genes outside every range are copied.  Genes need not be sorted by start.  Ranges
+ * must be ordered and disjoint inside [0, G); the coordinates of every gene of a range finite; W finite (else
+ * ICNV_E_BAD_ARG); G <= 2 097 120 (else ICNV_E_UNSUPPORTED).  NaN / Inf in X: ICNV_E_NONFINITE (the R wrapper falls back).
+ * The host builds the weights of every row (O(n^2) per range; sum over rows of (hi - lo + 1) doubles of device memory, up
+ * to the sum of n^2 when W spans whole ranges: ICNV_E_NOMEM if it does not fit).
+ * Arithmetic: t_k = fl(x_k w_k) as R's `*` (no contraction); den = sum(wv) in sequential long double, rounded (= R's on
+ * x86-64); the numerator N is Sum2 (cascaded two-sum) of the t_k in increasing k, and Y = fl(N / den).  With S = sum t_k,
+ * A = sum |t_k|, L = hi - lo + 1, u = 2^-53 and g_n = n u / (1 - n u):
+ *   |Y - S / den| <= ((2 u + u^2) |S| + (1 + u) g_{L-1}^2 A) / den,
+ * independent of the launch geometry; R's own value (80-bit partial sums, u' = 2^-64, g'_n = n u' / (1 - n u')) satisfies
+ * |Y_R - S / den| <= ((2 u + u^2) |S| + (1 + u)^2 g'_{L-1} A) / den.
+ * The dev variant takes X / Y on the device (leading dimensions ldx, ldy >= G; Y must not overlap X), the ranges and
+ * coordinates on the host; it returns once the result is complete. */
+ICNV_API int icnv_smooth_coordinates_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *chr_start,
+                                         const int32_t *chr_len, int K, const double *gene_start, const double *gene_stop,
+                                         double window_length);
+ICNV_API int icnv_dev_smooth_coordinates_f64(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C,
+                                             const int32_t *chr_start, const int32_t *chr_len, int K, const double *gene_start,
+                                             const double *gene_stop, double window_length, void *stream);
+
 /* Combine per-cell (sum, sd) pairs - e.g. all-gathered from several GPUs - into mu / sigma over all values
  * of those cells, in list order (what icnv_mean_sd_f64 does internally). */
 ICNV_API void icnv_combine_cell_stats(const double *sums, const double *sds, int64_t n, int64_t G, double *mu,

@@ -73,6 +73,8 @@ SIGNATURES = {
     "icnv_dev_bayesnet_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int,
                                       ct.c_uint64, _P, _P, _P, _P]),
     "icnv_debug_bayesnet": (c_int, [_P]),
+    "icnv_smooth_coordinates_f64": (c_int, [_P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, ct.c_double]),
+    "icnv_dev_smooth_coordinates_f64": (c_int, [_P, c_i64, _P, c_i64, c_i64, c_i64, _P, _P, c_int, _P, _P, ct.c_double, _P]),
     "icnv_dev_group_partial_sums_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, c_int, _P, _P]),
     "icnv_dev_combine_partials_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, _P]),
     "icnv_dev_bounds_from_partials_f64": (c_int, [_P, c_i64, c_int, c_i64, c_int, _P, _P, _P, _P, _P, _P]),

@@ -399,6 +399,31 @@ def runmean(X, k, chr_start=None, chr_len=None) -> np.ndarray:
     return Y
 
 
+def _coordinate_args(G, chr_start, chr_len, gene_start, gene_stop):
+    cs, cl = _i32(chr_start), _i32(chr_len)
+    st = np.ascontiguousarray(gene_start, dtype=np.float64)
+    sp = np.ascontiguousarray(gene_stop, dtype=np.float64)
+    if len(cs) != len(cl):
+        raise ValueError("chr_start and chr_len differ in length")
+    if st.shape != (G,) or sp.shape != (G,):
+        raise ValueError("gene_start and gene_stop need one entry per gene")
+    return cs, cl, st, sp
+
+
+def smooth_coordinates(X, chr_start, chr_len, gene_start, gene_stop, window_length) -> np.ndarray:
+    """smooth_by_chromosome_coordinates on the genes x cells matrix X with the row ranges (chr_start, chr_len) as its
+    chromosomes: every gene's value becomes the weighted mean over the genes within window_length of its midpoint, with
+    R's padding and recycling (icnv_smooth_coordinates_f64).  gene_start / gene_stop are per row of X.  Genes outside every
+    range, ranges of one gene and window_length < 2 are copied."""
+    X = _f64(X)
+    G, C = X.shape
+    cs, cl, st, sp = _coordinate_args(G, chr_start, chr_len, gene_start, gene_stop)
+    Y = np.empty_like(X, order="F")
+    _lib.check(_lib.load().icnv_smooth_coordinates_f64(_p(X), _p(Y), G, C, _p(cs), _p(cl), len(cs), _p(st), _p(sp),
+                                                       float(window_length)))
+    return Y
+
+
 def random_tree_heights(X, window=101, method="ward.D2", n_perm=100, seed=0, cells=None):
     """The permutation null of random-trees subclustering for the clade X[:, cells] (default: all columns) of the genes x
     cells matrix X: (merge, height, order, perm_max).  merge / height / order are the observed tree, runmean(window) ->

@@ -2121,3 +2121,67 @@ int icnv_debug_bayesnet(double *out4) {
 }
 
 }  // extern "C"
+
+// ---- coordinate-weighted smoothing (the kernel and the device body in icnv_smooth_coords.cu) --------------------------------
+// Weak reference, as for the linkage: a build without icnv_smooth_coords.cu reports it as unsupported.
+namespace icnv {
+int smooth_coords_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C, const int32_t *chr_start,
+                      const int32_t *chr_len, int K, const double *gene_start, const double *gene_stop, double W,
+                      cudaStream_t st, const char *who) __attribute__((weak));
+
+// Ranges ordered and disjoint inside [0, G); finite coordinates for every gene of a range; a finite window.
+static int smooth_coords_check(int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len, int K,
+                               const double *gene_start, const double *gene_stop, double W, const char *who) {
+    if (G <= 0 || C <= 0 || K < 0 || (K > 0 && (!chr_start || !chr_len)) || !gene_start || !gene_stop)
+        return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    if (G > (int64_t)65535 * 32 || G > INT32_MAX)
+        return set_error(ICNV_E_UNSUPPORTED, "%s: %lld genes (at most %d)", who, (long long)G, 65535 * 32);
+    if (!std::isfinite(W)) return set_error(ICNV_E_BAD_ARG, "%s: window_length is not finite", who);
+    for (int r = 0; r < K; ++r) {
+        const int64_t prev_end = r ? (int64_t)chr_start[r - 1] + chr_len[r - 1] : 0;
+        if (chr_len[r] < 0 || chr_start[r] < prev_end || (int64_t)chr_start[r] + chr_len[r] > G)
+            return set_error(ICNV_E_BAD_ARG, "%s: range %d [%d, +%d) is not ordered and disjoint inside [0, %lld)", who, r,
+                             chr_start[r], chr_len[r], (long long)G);
+        for (int64_t g = chr_start[r]; g < (int64_t)chr_start[r] + chr_len[r]; ++g)
+            if (!std::isfinite(gene_start[g]) || !std::isfinite(gene_stop[g]))
+                return set_error(ICNV_E_BAD_ARG, "%s: gene %lld has a non-finite start or stop", who, (long long)g);
+    }
+    return ICNV_OK;
+}
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_smooth_coordinates_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *chr_start,
+                                const int32_t *chr_len, int K, const double *gene_start, const double *gene_stop,
+                                double window_length) {
+    static const char *who = "icnv_smooth_coordinates_f64";
+    if (!icnv::smooth_coords_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no coordinate-smoothing kernel", who);
+    ICNV_HOST_PROLOGUE();
+    if (!X || !Y) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    int rc = icnv::smooth_coords_check(G, C, chr_start, chr_len, K, gene_start, gene_stop, window_length, who);
+    if (rc) return rc;
+    double *dX = nullptr, *dY = (double *)scratch(SLOT_OUT, sizeof(double) * (size_t)(G * C));
+    if (!dY) return ICNV_E_NOMEM;
+    if ((rc = upload_matrix_ring(X, G * C, &dX, st))) return rc;
+    if ((rc = icnv::smooth_coords_dev(dX, G, dY, G, G, C, chr_start, chr_len, K, gene_start, gene_stop, window_length, st, who)))
+        return rc;
+    ICNV_CUDA(cudaMemcpyAsync(Y, dY, sizeof(double) * (size_t)(G * C), cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return ICNV_OK;
+}
+
+int icnv_dev_smooth_coordinates_f64(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C,
+                                    const int32_t *chr_start, const int32_t *chr_len, int K, const double *gene_start,
+                                    const double *gene_stop, double window_length, void *stream) {
+    static const char *who = "icnv_dev_smooth_coordinates_f64";
+    if (!icnv::smooth_coords_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no coordinate-smoothing kernel", who);
+    ICNV_REQUIRE_READY();
+    if (!X || !Y || ldx < G || ldy < G) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    int rc = icnv::smooth_coords_check(G, C, chr_start, chr_len, K, gene_start, gene_stop, window_length, who);
+    if (rc) return rc;
+    return icnv::smooth_coords_dev(X, ldx, Y, ldy, G, C, chr_start, chr_len, K, gene_start, gene_stop, window_length,
+                                   pick_stream(stream), who);
+}
+
+}  // extern "C"

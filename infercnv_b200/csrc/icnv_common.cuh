@@ -177,6 +177,25 @@ __device__ __forceinline__ double u01(uint64_t h) {  // (0, 1]
 __device__ __forceinline__ double std_normal(uint64_t h1, uint64_t h2) {
     return sqrt(-2.0 * log(u01(h1))) * cospi(2.0 * u01(h2));
 }
+// Error-free transformations (the running mean, the DE means and variances, the coordinate smoother).
+// (s + e) == a + b exactly (no branch, no assumption on magnitudes)
+__device__ __forceinline__ void two_sum(double a, double b, double &s, double &e) {
+    s = a + b;
+    const double bp = s - a;
+    e = (a - (s - bp)) + (b - bp);
+}
+// (hi, lo) += x
+__device__ __forceinline__ void dd_add(double &hi, double &lo, double x) {
+    double s, e;
+    two_sum(hi, x, s, e);
+    two_sum(s, lo + e, hi, lo);
+}
+// (hi + lo) / c, c a positive integer: the quotient of hi and its exact remainder, corrected once
+__device__ __forceinline__ double dd_div(double hi, double lo, double c) {
+    const double q = hi / c;
+    const double r = fma(-q, c, hi);
+    return q + (r + lo) / c;
+}
 __device__ __forceinline__ double warp_min_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));

@@ -226,22 +226,6 @@ __global__ void __launch_bounds__(NT) pair_wilcox_kernel(const double *__restric
     }
 }
 
-// (s + e) == a + b exactly
-__device__ __forceinline__ void two_sum(double a, double b, double &s, double &e) {
-    s = a + b;
-    const double bp = s - a;
-    e = (a - (s - bp)) + (b - bp);
-}
-__device__ __forceinline__ void dd_add(double &hi, double &lo, double x) {
-    double s, e;
-    two_sum(hi, x, s, e);
-    two_sum(s, lo + e, hi, lo);
-}
-__device__ __forceinline__ double dd_div(double hi, double lo, double c) {
-    const double q = hi / c;
-    const double r = fma(-q, c, hi);
-    return q + (r + lo) / c;
-}
 // block double-double sum in a fixed tree order; every thread gets hi + lo as (hi, lo)
 __device__ void block_dd_sum(double &hi, double &lo, double *sh) {
     __syncthreads();

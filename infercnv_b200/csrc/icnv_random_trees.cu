@@ -46,25 +46,6 @@ namespace rt {
 constexpr int RM_NT = 128;
 constexpr int PG_NT = 256;
 
-// s + e == a + b exactly (no branch, no assumption on magnitudes)
-__device__ __forceinline__ void two_sum(double a, double b, double &s, double &e) {
-    s = a + b;
-    const double bp = s - a;
-    e = (a - (s - bp)) + (b - bp);
-}
-// (hi, lo) += x
-__device__ __forceinline__ void dd_add(double &hi, double &lo, double x) {
-    double s, e;
-    two_sum(hi, x, s, e);
-    two_sum(s, lo + e, hi, lo);
-}
-// (hi + lo) / c, c a positive integer: the quotient of hi and its exact remainder, corrected once
-__device__ __forceinline__ double dd_div(double hi, double lo, double c) {
-    const double q = hi / c;
-    const double r = fma(-q, c, hi);
-    return q + (r + lo) / c;
-}
-
 // One column range [s, s + L) of x -> y.
 __device__ void runmean_range(const double *x, double *y, int64_t L, int k) {
     const int64_t kk = k < L ? k : L;

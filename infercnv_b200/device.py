@@ -446,6 +446,22 @@ class Engine:
         m = merge.cpu().numpy().T
         return m, height.cpu().numpy(), hclust_order(m), perm_max.cpu().numpy()
 
+    def smooth_coordinates(self, X, chr_start, chr_len, gene_start, gene_stop, window_length, out=None):
+        """smooth_by_chromosome_coordinates on the resident (C, G) float64 tensor X with contiguous genes, as
+        api.smooth_coordinates and bit-identical to it: returns Y (C, G), `out` or a new tensor (never X itself)."""
+        from .api import _coordinate_args
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X.shape
+        cs, cl, st, sp = _coordinate_args(G, chr_start, chr_len, gene_start, gene_stop)
+        Y = torch.empty_like(X) if out is None else out
+        if Y.data_ptr() == X.data_ptr():
+            raise ValueError("out must not be X: every output reads its neighbours' inputs")
+        _lib.check(self.lib.icnv_dev_smooth_coordinates_f64(
+            X.data_ptr(), max(X.stride(0), G), Y.data_ptr(), max(Y.stride(0), G), G, C, cs.ctypes.data, cl.ctypes.data,
+            len(cs), st.ctypes.data, sp.ctypes.data, float(window_length), _stream_ptr()))
+        return Y
+
     def mask_non_de(self, X, ref_groups, subclusters, test="wilcoxon", p_val_thresh=0.05, rule="any", center_val=None,
                     jitter_mean=1e-4, jitter_sd=1e-4, seed=0, out=None):
         """mask_non_DE_genes_basic on the resident (C, G) float64 tensor X (single GPU), as api.mask_non_de_genes: returns

@@ -529,6 +529,37 @@ b200_smooth_by_chromosome_runmeans <- function(infercnv_obj, window_length) {
     infercnv_obj
 }
 
+## smooth_by_chromosome_coordinates (R/inferCNV_ops.R:2534-2622), run()'s step 10 for smooth_method = "coordinates": every
+## chromosome's genes smoothed by the genomic-distance weights of .smooth_helper_by_coordinates in one GPU call, chromosomes
+## of one gene left alone, hspike mirrored with window_length = 51 as in the original.  Falls back for NA, a non-double /
+## non-matrix slot, genes of a chromosome not contiguous, NA or non-finite start / stop, a window_length that is not one
+## finite number, window_length < 2 (the original's warnings), or a library error.
+b200_smooth_by_chromosome_coordinates <- function(infercnv_obj, window_length) {
+    orig <- .icnv_env$orig$smooth_by_chromosome_coordinates
+    m <- infercnv_obj@expr.data
+    codes <- .icnv_chr_codes(infercnv_obj)
+    gs <- infercnv_obj@gene_order[["start"]]
+    ge <- infercnv_obj@gene_order[["stop"]]
+    if (!.icnv_enabled() || !.icnv_ok(m) || is.null(codes) || !is.numeric(gs) || !is.numeric(ge) ||
+        length(gs) != nrow(m) || length(ge) != nrow(m) || !all(is.finite(gs)) || !all(is.finite(ge)) ||
+        !is.numeric(window_length) || length(window_length) != 1 || !is.finite(window_length) || window_length < 2)
+        return(orig(infercnv_obj, window_length))
+    r <- rle(codes)
+    lens <- as.integer(r$lengths)
+    starts <- as.integer(c(0L, cumsum(lens)[-length(lens)]))
+    for (chr in unique(infercnv_obj@gene_order[["chr"]])) futile.logger::flog.info(paste0("smooth_by_chromosome: chr: ", chr))
+    res <- .icnv_try(.Call("icnvR_smooth_coordinates", m, starts, lens, as.double(gs), as.double(ge), as.double(window_length)),
+                     "smooth_by_chromosome_coordinates")
+    if (is.null(res)) return(orig(infercnv_obj, window_length))
+    dimnames(res) <- dimnames(m)
+    infercnv_obj@expr.data <- res
+    if (!is.null(infercnv_obj@.hspike)) {
+        futile.logger::flog.info("-mirroring for hspike")
+        infercnv_obj@.hspike <- b200_smooth_by_chromosome_coordinates(infercnv_obj@.hspike, window_length = 51)
+    }
+    infercnv_obj
+}
+
 ## .parameterize_random_cluster_heights_smoothed_trees (R/inferCNV_tumor_subclusters.random_smoothed_trees.R:217-304): the
 ## observed tree and the 100 permuted maxima of one clade in one GPU call, the same list(h_obs, max_h,
 ## rand_max_height_dist, ecdf).  h_obs is the "hclust" object b200_hclust returns (labels = colnames(expr_matrix)).  The
@@ -753,7 +784,7 @@ infercnvb200_install <- function() {
              "get_predicted_CNV_regions", "remove_outliers_norm", "clear_noise",
              "predict_CNV_via_HMM_on_tumor_subclusters_per_chr", "i3HMM_predict_CNV_via_HMM_on_tumor_subclusters",
              "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
-             "mask_non_DE_genes_basic", "inferCNVBayesNet",
+             "mask_non_DE_genes_basic", "inferCNVBayesNet", "smooth_by_chromosome_coordinates",
              ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
              ".parameterize_random_cluster_heights_smoothed_trees")
     ns <- asNamespace("infercnv")

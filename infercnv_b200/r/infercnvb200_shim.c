@@ -272,6 +272,24 @@ SEXP icnvR_runmean(SEXP expr, SEXP chr_start, SEXP chr_len, SEXP k) {
     return ans;
 }
 
+/* smooth_by_chromosome_coordinates (ops.R:2534-2622) with the ranges the R closure computed (0-based starts, lengths) and
+ * gene_order's start / stop as doubles, one per row of expr. */
+SEXP icnvR_smooth_coordinates(SEXP expr, SEXP chr_start, SEXP chr_len, SEXP gene_start, SEXP gene_stop, SEXP window_length) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int K = Rf_length(chr_start);
+    if (Rf_length(chr_len) != K) Rf_error("infercnv_b200: coordinate-smoothing ranges differ in length");
+    if (Rf_length(gene_start) != G || Rf_length(gene_stop) != G)
+        Rf_error("infercnv_b200: coordinate smoothing needs one start and stop per gene");
+    SEXP ans = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    int rc = icnv_smooth_coordinates_f64(REAL(expr), REAL(ans), G, C, (const int32_t *)INTEGER(chr_start),
+                                         (const int32_t *)INTEGER(chr_len), K, REAL(gene_start), REAL(gene_stop),
+                                         Rf_asReal(window_length));
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* .parameterize_random_cluster_heights_smoothed_trees (random_smoothed_trees.R:217-304) on the clade matrix expr (genes x
  * cells): list(merge, height, order, rand_max_height_dist); the closure builds the "hclust" object.  seed: two whole numbers
  * in [0, 2^31) drawn from R's RNG, combined as hi * 2^32 + lo. */
@@ -581,6 +599,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_random_tree_heights", (DL_FUNC)&icnvR_random_tree_heights, 5},
     {"icnvR_mask_non_de", (DL_FUNC)&icnvR_mask_non_de, 8},
     {"icnvR_bayesnet", (DL_FUNC)&icnvR_bayesnet, 10},
+    {"icnvR_smooth_coordinates", (DL_FUNC)&icnvR_smooth_coordinates, 6},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

@@ -181,6 +181,25 @@ def smooth_by_chromosome(infercnv_obj: Infercnv, window_length: int, smooth_ends
     return obj
 
 
+def smooth_by_chromosome_coordinates(infercnv_obj: Infercnv, window_length: float) -> Infercnv:
+    """R/inferCNV_ops.R:2534-2622: every gene's value becomes the weighted mean over the genes of its chromosome within
+    window_length of its midpoint (gene_order_start / gene_order_stop), with R's padding and recycling; the hidden spike is
+    mirrored with window_length = 51 as in the original."""
+    obj = copy.copy(infercnv_obj)
+    if obj.gene_order_start is None or obj.gene_order_stop is None:
+        raise ValueError("smooth_by_chromosome_coordinates needs gene_order_start and gene_order_stop")
+    cs, cl = obj.chr_ranges()
+    for s, n in zip(cs, cl):
+        log.info("smooth_by_chromosome: chr: %s", _chr_label(obj, obj.gene_order_chr[s]))
+        if n > 1 and window_length < 2:
+            log.warning("window length < 2, returning original unmodified data")      # ops.R:2568-2571
+    obj.expr_data = api.smooth_coordinates(obj.expr_data, cs, cl, obj.gene_order_start, obj.gene_order_stop, window_length)
+    if obj.hspike is not None:
+        log.info("-mirroring for hspike")
+        obj.hspike = smooth_by_chromosome_coordinates(obj.hspike, window_length=51)
+    return obj
+
+
 def center_cell_expr_across_chromosome(infercnv_obj: Infercnv, method: str = "mean") -> Infercnv:
     """R/inferCNV_ops.R:2074-2088; any method other than "median" centres by the mean (:2096-2107)."""
     log.info("::center_smooth across chromosomes per cell")
