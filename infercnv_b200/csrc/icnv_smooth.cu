@@ -194,6 +194,7 @@ constexpr int CAND_MAX = 64;   // candidates ranked directly at the end of the s
 
 __device__ unsigned long long g_stats[16];  // [0] median rounds, [1] medians, [2] split exits, [3] gather exits,
                                             // [4..9] cycles spent by CTA 0 in: wait, A, B scans, B outputs, C median, D
+                                            // (ICNV_STAGE_TIMERS builds), [10] medians found by the histogram
 
 // ---- block-wide reductions with one __syncthreads each (double-buffered scratch) ----------------
 template <int NW>
@@ -593,65 +594,97 @@ __device__ __forceinline__ double block_median_smem(const double *__restrict__ v
     return (cand[CAND_MAX] + cand[CAND_MAX + 1]) * 0.5;   // cand is next touched a whole cell (many barriers) later
 }
 
-// ---- median by one histogram pass ----------------------------------------------------------------
-// |mean - median| <= sd for any distribution, so the HIST_NB equal-width bins spanning mean +- sd hold both middle
-// order statistics.  bin(v) = low word of fma(v, scale, C) with C = 1.5*2^52 - (mean - sd)*scale is a monotone
-// function of v evaluated by the same instruction in both passes, so "values in lower bins" are exactly the values
-// ranked below the bin: pass 1 counts (shared-memory atomics for the inner bins, a register for "below"), a
-// block-wide scan finds the bin(s) holding ranks kA and kB, pass 2 gathers those bins' values (<= CAND_MAX,
-// otherwise the bracketing selection above takes over) and they are ranked directly.  Two passes over the
-// values, any thread reads any value: both passes use the coalesced 16-byte mapping.
+// ---- median by a histogram counted while the values are produced ---------------------------------
+// HIST_NB equal-width bins span mean(x') +- HIST_SPAN sd(x') of the stage-A output x'.  Its sum and sum of squares come out
+// of the first scan pass of stage B (the slice totals it forms anyway, and one FMA per gene), so the bins are placed before
+// the first smoothed value exists and stage B's output loops count each value as they store it - no separate counting
+// pass over the column, and no reduction over the smoothed values.  The
+// pyramid weights are normalised, so the smoothed column keeps the mean of x' (up to the renormalised chromosome ends)
+// with a smaller spread, and its median sits far inside the span for any column with a centre; nothing depends on that:
+//   bin(v) = low word of fma(v, scale, C), C = 1.5*2^52 - (mean - HIST_SPAN sd) scale, is a monotone function of v, and the
+// counting (hist_count) and the gathering pass evaluate it with the same fma on the same operands, so "values in lower
+// bins" are exactly the values ranked below the bin.  Counting: shared-memory atomics for the bins inside the span, a
+// register for "below".  A block-wide scan finds the bin(s) holding ranks kA and kB, one pass gathers those bins' values
+// and they are ranked directly: the centre is the exact median.  Whenever the estimate fails - a middle rank outside the
+// span, more than CAND_MAX values in the middle bin(s), no variance, a non-finite value - the bracketing selection above
+// takes over.
+// HIST_SPAN: on the benchmark's columns (100 000 x 10 000, window 101) |median - mean(x')| <= 0.1 sd(x') and sd(smoothed) =
+// 0.10 .. 0.43 sd(x'); a quarter of sd(x') either side leaves 10 (median) .. 33 (most) candidates of the CAND_MAX allowed.
 constexpr int HIST_NB = 2048;
+constexpr float HIST_SPAN = 0.25f;
+constexpr int HIST_HI0 = 0x43380000;   // high word of 1.5*2^52 + k, 0 <= k < 2^32: k is the low word
 
-// n = number of (finite) values, n_slots = slots of `vals` to walk (>= n; the extra slots hold +inf and are neither
-// counted nor gathered).
+// this warp's share of the sum / sum of squares of x', ahead of the barrier behind the first scan pass
+template <int NW>
+__device__ __forceinline__ void hist_stats_put(Red<NW> &r, int phase, double s1, double s2) {
+    s1 = warp_sum_d(s1);
+    s2 = warp_sum_d(s2);
+    if ((threadIdx.x & 31) == 0) {
+        r.d[phase][0][threadIdx.x >> 5] = s1;
+        r.d[phase][1][threadIdx.x >> 5] = s2;
+    }
+}
+
+// Behind that barrier: warp 0 folds the shares and leaves (scale, C) in geo[0..1] - read by every thread behind a later
+// barrier, so all of them and both passes bin identically; scale = 0 means "no histogram for this cell".  The median never
+// depends on the geometry (the candidates are ranked exactly), so cheap arithmetic places it: a single-precision reciprocal
+// square root instead of two divisions and a square root in double precision.
+template <int NW, int NB>
+__device__ __forceinline__ void hist_geometry(Red<NW> &r, int &phase, int n, double inv_n, double *geo) {
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x < 32) {
+        const double S1 = warp_sum_d((lane < NW) ? r.d[phase][0][lane] : 0.0);
+        const double S2 = warp_sum_d((lane < NW) ? r.d[phase][1][lane] : 0.0);
+        const double mean = S1 * inv_n;
+        const double var = fma(S2, inv_n, -mean * mean);
+        double scale = 0.0, C = 0.0;
+        if (var > 0.0 && n > 4 * CAND_MAX) {   // (a NaN or an infinity in x' leaves var NaN)
+            const float rs = rsqrtf((float)var);
+            const double half = var * (double)(rs * HIST_SPAN);   // HIST_SPAN sd
+            const double sc = (double)(rs * (0.5f * NB / HIST_SPAN));
+            if (sc < 1e290 && sc > 0.0) {   // otherwise var is outside the single-precision range
+                scale = sc;
+                C = fma(half - mean, sc, 6755399441055744.0);   // 1.5 * 2^52
+            }
+        }
+        if (lane == 0) {
+            geo[0] = scale;
+            geo[1] = C;
+        }
+    }
+    phase ^= 1;
+}
+
+// One value into the histogram.  Values outside the span count into this lane's own spare word behind the tables (never
+// read; per lane, so that a warp does not pile onto one address): one unconditional atomic per value instead of a branch.
+template <int NB>
+__device__ __forceinline__ void hist_count(double v, double scale, double C, int *hist, unsigned dump, int &below) {
+    const double t = fma(v, scale, C);
+    const int hi = __double2hiint(t);
+    const unsigned lo = (unsigned)__double2loint(t);
+    atomicAdd(&hist[(hi == HIST_HI0 && lo < (unsigned)NB) ? lo : dump], 1);
+    below += (hi < HIST_HI0) ? 1 : 0;
+}
+
+// The histogram of the n (finite) values is complete and wcnt[w] holds warp w's count of values below the first bin.
+// n_slots = slots of `vals` to walk (>= n; the extra slots hold +inf and are never gathered).
 template <int NT, int NB = HIST_NB>
-__device__ __forceinline__ bool block_median_hist(const double *__restrict__ vals, int n, double inv_n, double S1, double S2, int *hist, int dump_off,
+__device__ __forceinline__ bool block_median_hist(const double *__restrict__ vals, int n, double scale, double C, int *hist,
                                                   int *hres, int *wcnt, double *cand, int *cand_n, double &result, int n_slots = 0) {
     constexpr int NW = NT / 32;
     constexpr int BPT = NB / NT;   // bins scanned per thread
     static_assert(NB % NT == 0 && BPT >= 1 && BPT <= 8, "the bin count must be a small multiple of NT");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const unsigned dump = (unsigned)(dump_off + lane);   // index (relative to hist) of this lane's spare word
     const int kA = (n - 1) >> 1, kB = n >> 1;
-    // Bin geometry in cheap arithmetic: every thread evaluates the same instruction sequence, so all of them and both
-    // passes bin with identical scale / C, and the median itself never depends on them (the candidates are ranked exactly) -
-    // a single-precision reciprocal square root is enough for "about mean +- sd".  ~25 instead of ~100 instructions per
-    // thread and cell (two divisions, a square root and a third division in double precision before).
-    const double mean = S1 * inv_n;
-    const double var = fma(S2, inv_n, -mean * mean);
-    if (!(var > 0.0) || n <= 4 * CAND_MAX) return false;
-    const float rs = rsqrtf((float)var);
-    const double sd = var * (double)rs;
-    const double scale = (double)(rs * (0.5f * NB));
-    if (!(scale < 1e290) || !(scale > 0.0)) return false;   // var outside the single-precision range: bracketing selection
-    const double MAGIC = 6755399441055744.0;   // 1.5 * 2^52: integers 0 .. 2^32-1 land in the low word, high word HI0
-    constexpr int HI0 = 0x43380000;
-    const double C = fma(sd - mean, scale, MAGIC);
+    if (!(scale > 0.0)) return false;   // nothing was binned
+    constexpr int HI0 = HIST_HI0;
     if (tid == 0) {
         hres[0] = -1;
         hres[2] = -1;
         *cand_n = 0;
     }
     const double2 *v2 = reinterpret_cast<const double2 *>(vals);
-    const int n2 = ((n_slots > 0 ? n_slots : n) + 1) >> 1;   // an odd n is padded with +inf (never counted, never gathered)
-    int cb = 0;
-#pragma unroll 2
-    for (int i = tid; i < n2; i += NT) {
-        const double2 v = v2[i];
-        const double tx = fma(v.x, scale, C), ty = fma(v.y, scale, C);
-        const int hx = __double2hiint(tx), hy = __double2hiint(ty);
-        const unsigned lx = (unsigned)__double2loint(tx), ly = (unsigned)__double2loint(ty);
-        // values outside mean +- sd count into this lane's own spare word behind the tables (never read; per lane, so that
-        // a third of the warp does not pile onto one address): one unconditional atomic per value instead of a branch around it
-        atomicAdd(&hist[(hx == HI0 && lx < (unsigned)NB) ? lx : dump], 1);
-        atomicAdd(&hist[(hy == HI0 && ly < (unsigned)NB) ? ly : dump], 1);
-        cb += (hx < HI0) ? 1 : 0;
-        cb += (hy < HI0) ? 1 : 0;
-    }
-    cb = __reduce_add_sync(0xffffffffu, cb);
-    if (lane == 0) wcnt[warp] = cb;
-    __syncthreads();   // histogram complete
+    const int n2 = ((n_slots > 0 ? n_slots : n) + 1) >> 1;   // an odd n is padded with +inf (never gathered)
     int cnt[BPT];
     int s = 0;
 #pragma unroll
@@ -754,15 +787,17 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
     double *zslot = rext + (PADQ ? 0 : p.K * p.h);           // a 0.0 the edge loads can point at (Q before the start)
     unsigned long long *bar = reinterpret_cast<unsigned long long *>(zslot + 2);
     int *hist = reinterpret_cast<int *>(bar + 2);            // HIST_NB bins, zero between cells
-    int *hres = hist + HIST_NB;                              // 4 results of the bin search (+4 spare)
+    int *hres = hist + HIST_NB;                              // 4 results of the bin search
+    double *hgeo = reinterpret_cast<double *>(hres + 4);     // bin geometry of the current cell (hist_geometry)
     int *wcnt = hres + 8;                                    // [2][NW]
     int *cand_n = wcnt + 2 * NW;
     int *chr_cs = cand_n + 2;                                // PADQ: [K] chromosome start, [K] chromosome length
     int *chr_n = chr_cs + p.K;
-    int *hdump = chr_n + p.K;                                // [32] per-lane spare words of the histogram pass
+    int *hdump = chr_n + p.K;                                // [32] per-lane spare words of the histogram counting
     double *const sm = reinterpret_cast<double *>(smem_raw); // everything below is indexed relative to this
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned dump = (unsigned)((int)(hdump - hist) + lane);   // index (relative to hist) of this lane's spare word
     const int G = (int)p.G;
     const int h = p.h;
     const bool do_smooth = p.window >= 2;
@@ -778,8 +813,9 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
     if (tid == 0) {
         mbar_init(bar, 1);
         zslot[0] = 0.0;
-        buf0[p.s_elems - 1] = INFINITY;   // pad of an odd G: never counted by the median (overwritten when G is even)
+        buf0[p.s_elems - 1] = INFINITY;   // pad of an odd G: never gathered by the median (overwritten when G is even)
         buf1[p.s_elems - 1] = INFINITY;
+        hgeo[0] = hgeo[1] = 0.0;          // without median centring nothing is binned
     }
     for (int i = tid; i < HIST_NB; i += NT) hist[i] = 0;
     for (int i = tid; i < 128; i += NT) {
@@ -879,20 +915,39 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
 
         // ---- B: pyramid smooth oth (x') -> in (smoothed) -------------------------------------------------
         const double *xs = oth + a0;
-        double ys1 = 0.0, ys2 = 0.0;   // sum / sum of squares of this thread's outputs (first median pivots)
+        double ys1 = 0.0;      // sum of this thread's outputs (mean centring)
+        double hscale, hC;     // bin geometry of the histogram median (hist_geometry)
+        int cb = 0;            // this thread's outputs below the first bin
         if (!do_smooth) {
+            if (p.center == 1) {
+                double t1 = 0.0, t2 = 0.0;
+                for (int q = 0; q < len; ++q) {
+                    t1 += xs[q];
+                    t2 = fma(xs[q], xs[q], t2);
+                }
+                hist_stats_put<NW>(red, phase, t1, t2);
+                __syncthreads();
+                hist_geometry<NW, HIST_NB>(red, phase, G, inv_G, hgeo);
+                __syncthreads();
+            }
+            hscale = hgeo[0];
+            hC = hgeo[1];
             for (int q = 0; q < len; ++q) {
                 const double out = xs[q];
                 if (!PADQ) in[a0 + q] = out;
                 ys1 += out;
-                ys2 = fma(out, out, ys2);
+                hist_count<HIST_NB>(out, hscale, hC, hist, dump, cb);
             }
         } else {
             // pass 1: segment total of x
-            double tot = 0.0;
+            double tot = 0.0, tot2 = 0.0;   // tot2: sum of squares, for the bin geometry of the median (hist_geometry)
 #pragma unroll(FIX ? LFIX : 4)
             for (int q = 0; q < (FIX ? LFIX : len); ++q)
-                if (!FIX || q < len) tot += xs[q];
+                if (!FIX || q < len) {
+                    tot += xs[q];
+                    tot2 = fma(xs[q], xs[q], tot2);
+                }
+            if (p.center == 1) hist_stats_put<NW>(red, phase, tot, tot2);
             double inc = tot;
 #pragma unroll
             for (int d = 1; d < 32; d <<= 1) {
@@ -903,6 +958,7 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
             if (lane <= lane_first) exc = 0.0;
             if (lane == 31) tails[warp] = inc;
             __syncthreads();
+            if (p.center == 1) hist_geometry<NW, HIST_NB>(red, phase, G, inv_G, hgeo);   // warp 0; read behind the next barriers
             double carry = 0.0;
             for (int u = wfirst; u < warp; ++u) carry += tails[u];
             const double offP = exc + carry;   // P just before this segment
@@ -969,6 +1025,8 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
             }
             __syncthreads();
             lap(2);
+            hscale = hgeo[0];
+            hC = hgeo[1];
             // outputs: N(j) = (Q(j+h) - Q(j-1)) - (Q(j-1) - Q(j-h-2)), one code path for interior and edge genes -
             // out-of-range Q come from the pads (PADQ) or, by index selection, from the continuation table / the zero slot
             if (n >= 2 && PADQ) {
@@ -988,7 +1046,7 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
                         pI += dI;
                         O[q] = out;
                         ys1 += out;
-                        ys2 = fma(out, out, ys2);
+                        hist_count<HIST_NB>(out, hscale, hC, hist, dump, cb);
                     }
                 } else {
                     for (int q = 0; q < len; ++q) {
@@ -1006,7 +1064,7 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
                         }
                         O[q] = out;
                         ys1 += out;
-                        ys2 = fma(out, out, ys2);
+                        hist_count<HIST_NB>(out, hscale, hC, hist, dump, cb);
                     }
                 }
             } else if (n >= 2) {
@@ -1033,7 +1091,7 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
                     }
                     in[a0 + q] = out;
                     ys1 += out;
-                    ys2 = fma(out, out, ys2);
+                    hist_count<HIST_NB>(out, hscale, hC, hist, dump, cb);
                 }
             } else {
                 // single-gene chromosome: left untouched (ops.R:2417); Q of a single element is the element, and with
@@ -1042,22 +1100,19 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
                     const double out = oth[a0 + q];
                     if (!PADQ) in[a0 + q] = out;
                     ys1 += out;
-                    ys2 = fma(out, out, ys2);
+                    hist_count<HIST_NB>(out, hscale, hC, hist, dump, cb);
                 }
             }
         }
-        ys1 = warp_sum_d(ys1);
-        ys2 = warp_sum_d(ys2);
-        if (lane == 0) {
-            red.d[phase][0][warp] = ys1;
-            red.d[phase][1][warp] = ys2;
+        if (p.center == 1) {
+            cb = __reduce_add_sync(0xffffffffu, cb);
+            if (lane == 0) wcnt[warp] = cb;
+        } else if (p.center == 2) {
+            ys1 = warp_sum_d(ys1);
+            if (lane == 0) red.d[phase][0][warp] = ys1;
         }
-        __syncthreads();   // smoothed values complete in `in` (PADQ: in `oth`); Q no longer needed
+        __syncthreads();   // smoothed values complete in `in` (PADQ: in `oth`), their histogram too; Q no longer needed
         double *const sv = PADQ ? oth : in;   // the smoothed column stages C and D read
-        double S1 = (lane < NW) ? red.d[phase][0][lane] : 0.0, S2 = (lane < NW) ? red.d[phase][1][lane] : 0.0;
-        S1 = warp_sum_d(S1);
-        S2 = warp_sum_d(S2);
-        phase ^= 1;
         lap(3);
         if (tid == 0) {    // next cell's column lands where Q was (`oth`; PADQ: `in`) while the median and the epilogue run
             const int64_t cn = ci + gridDim.x;
@@ -1075,7 +1130,7 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
         double centre = 0.0;
         if (p.center == 1) {
             if (tid == 0) atomicAdd(&g_stats[1], 1ull);
-            if (block_median_hist<NT>(sv, G, inv_G, S1, S2, hist, (int)(hdump - hist), hres, wcnt, cand, cand_n, centre)) {
+            if (block_median_hist<NT>(sv, G, hscale, hC, hist, hres, wcnt, cand, cand_n, centre)) {
                 if (tid == 0) atomicAdd(&g_stats[10], 1ull);
             } else {   // tiny or degenerate columns, > CAND_MAX ties in the middle bin: bracketing selection
                 double s1 = 0.0, s2 = 0.0;
@@ -1087,6 +1142,8 @@ __global__ void __launch_bounds__(NT, 1) cell_pipeline3_kernel(const CellParams 
                 centre = block_median_smem<NT>(sv, a0, len, G, s1, s2, red, phase, cand, cand_n);
             }
         } else if (p.center == 2) {
+            const double S1 = warp_sum_d((lane < NW) ? red.d[phase][0][lane] : 0.0);
+            phase ^= 1;
             centre = S1 / (double)G;
         }
 
@@ -1215,13 +1272,15 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
     // whenever h is odd - the offsets in front of it are h + 2 plus even counts of doubles)
     int4 *ctab = reinterpret_cast<int4 *>((reinterpret_cast<uintptr_t>(bar + 2) + 15) & ~(uintptr_t)15);
     int *hist = reinterpret_cast<int *>(ctab + p.n_chunks);   // NB bins, zero between cells
-    int *hres = hist + NB;
+    int *hres = hist + NB;                                    // 4 results of the bin search
+    double *hgeo = reinterpret_cast<double *>(hres + 4);      // bin geometry of the current cell (hist_geometry)
     int *wcnt = hres + 8;                                     // [2][NW]
     int *cand_n = wcnt + 2 * NW;
-    int *hdump = cand_n + 2;                                  // [32] per-lane spare words of the histogram pass
+    int *hdump = cand_n + 2;                                  // [32] per-lane spare words of the histogram counting
     Chr4 *chr = reinterpret_cast<Chr4 *>(hdump + 32);         // [K + 1]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned dump = (unsigned)((int)(hdump - hist) + lane);   // index (relative to hist) of this lane's spare word
     const int G = (int)p.G, h = p.h, K = p.K, nb = p.nb, NCH = p.n_chunks;
     const bool do_smooth = p.window >= 2;
     const int sh = do_smooth ? h + 2 : 0;   // smoothed values sit this many slots below x' / Q
@@ -1232,7 +1291,10 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
         const double full = (double)(h + 1) * (double)(h + 1);
         for (int r = tid; r <= h; r += NT) invD[r] = 1.0 / (full - 0.5 * (double)r * (double)(r + 1));
     }
-    if (tid == 0) mbar_init(bar, 1);
+    if (tid == 0) {
+        mbar_init(bar, 1);
+        hgeo[0] = hgeo[1] = 0.0;   // without median centring nothing is binned
+    }
     for (int i = tid; i < NB; i += NT) hist[i] = 0;
     for (int i = tid; i < 128; i += NT) {
         ltab[i] = make_double2(g_log_tab[i][0], g_log_tab[i][1]);
@@ -1349,21 +1411,40 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
         __syncthreads();
 
         // ---- B: pyramid smooth in place --------------------------------------------------------------------------------------
-        double ys1 = 0.0, ys2 = 0.0;   // sum / sum of squares of the outputs (bin geometry of the median)
+        double ys1 = 0.0;      // sum of the outputs (mean centring)
+        double hscale, hC;     // bin geometry of the histogram median (hist_geometry)
+        int cb = 0;            // this thread's outputs below the first bin
         if (!do_smooth) {
             const double *xs = buf + my_fb;
+            if (p.center == 1) {
+                double t1 = 0.0, t2 = 0.0;
+                for (int q = 0; q < len; ++q) {
+                    t1 += xs[q];
+                    t2 = fma(xs[q], xs[q], t2);
+                }
+                hist_stats_put<NW>(red, phase, t1, t2);
+                __syncthreads();
+                hist_geometry<NW, NB>(red, phase, G, inv_G, hgeo);
+                __syncthreads();
+            }
+            hscale = hgeo[0];
+            hC = hgeo[1];
             for (int q = 0; q < len; ++q) {
                 const double out = xs[q];
                 ys1 += out;
-                ys2 = fma(out, out, ys2);
+                hist_count<NB>(out, hscale, hC, hist, dump, cb);
             }
         } else {
             double *xs = buf + my_vb;
             // pass 1: slice total of x
-            double tot = 0.0;
+            double tot = 0.0, tot2 = 0.0;   // tot2: sum of squares, for the bin geometry of the median (hist_geometry)
 #pragma unroll(FIX ? LFIX : 4)
             for (int q = 0; q < (FIX ? LFIX : len); ++q)
-                if (!FIX || q < len) tot += xs[q];
+                if (!FIX || q < len) {
+                    tot += xs[q];
+                    tot2 = fma(xs[q], xs[q], tot2);
+                }
+            if (p.center == 1) hist_stats_put<NW>(red, phase, tot, tot2);
             double inc = tot;
 #pragma unroll
             for (int d = 1; d < 32; d <<= 1) {
@@ -1374,6 +1455,7 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
             if (lane <= lane_first) exc = 0.0;
             if (lane == 31) tails[warp] = inc;
             __syncthreads();
+            if (p.center == 1) hist_geometry<NW, NB>(red, phase, G, inv_G, hgeo);   // warp 0; read behind the next barriers
             double carry = 0.0;
             for (int u = wfirst; u < warp; ++u) carry += tails[u];
             const double offP = exc + carry;   // P just before this slice
@@ -1428,6 +1510,8 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
                 }
             }
             __syncthreads();
+            hscale = hgeo[0];
+            hC = hgeo[1];
             // outputs, V4_R chunks per warp and round
             for (int it0 = 0; it0 < n_it_cta; it0 += V4_R) {   // the same number of rounds (barriers) in every warp
                 double o[V4_R];
@@ -1446,7 +1530,7 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
                             o[r] = out;
                             wpos[r] = d.x + lane - sh;
                             ys1 += out;
-                            ys2 = fma(out, out, ys2);
+                            hist_count<NB>(out, hscale, hC, hist, dump, cb);
                         } else if (lane < d.z) {
                             const int c = d.w & 0xffff;
                             const int nc = chr[c].n, j = d.y + lane - chr[c].cs;
@@ -1468,7 +1552,7 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
                             o[r] = out;
                             wpos[r] = d.x + lane - sh;
                             ys1 += out;
-                            ys2 = fma(out, out, ys2);
+                            hist_count<NB>(out, hscale, hC, hist, dump, cb);
                         }
                     }
                 }
@@ -1486,23 +1570,20 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
                 for (int e = f2 + lane; e < f3; e += 32) buf[e] = INFINITY;
             }
         }
-        ys1 = warp_sum_d(ys1);
-        ys2 = warp_sum_d(ys2);
-        if (lane == 0) {
-            red.d[phase][0][warp] = ys1;
-            red.d[phase][1][warp] = ys2;
+        if (p.center == 1) {
+            cb = __reduce_add_sync(0xffffffffu, cb);
+            if (lane == 0) wcnt[warp] = cb;
+        } else if (p.center == 2) {
+            ys1 = warp_sum_d(ys1);
+            if (lane == 0) red.d[phase][0][warp] = ys1;
         }
-        __syncthreads();   // smoothed values complete at frame start + j
-        double S1 = (lane < NW) ? red.d[phase][0][lane] : 0.0, S2 = (lane < NW) ? red.d[phase][1][lane] : 0.0;
-        S1 = warp_sum_d(S1);
-        S2 = warp_sum_d(S2);
-        phase ^= 1;
+        __syncthreads();   // smoothed values complete at frame start + j, their histogram too
 
         // ---- C: per-cell centre --------------------------------------------------------------------------------------------
         double centre = 0.0;
         if (p.center == 1) {
             if (tid == 0) atomicAdd(&g_stats[1], 1ull);
-            if (block_median_hist<NT, NB>(buf, G, inv_G, S1, S2, hist, (int)(hdump - hist), hres, wcnt, cand, cand_n, centre, nb)) {
+            if (block_median_hist<NT, NB>(buf, G, hscale, hC, hist, hres, wcnt, cand, cand_n, centre, nb)) {
                 if (tid == 0) atomicAdd(&g_stats[10], 1ull);
             } else {   // tiny or degenerate columns, > CAND_MAX ties in the middle bin: bracketing selection
                 double s1 = 0.0, s2 = 0.0;
@@ -1514,6 +1595,8 @@ __global__ void __launch_bounds__(NT, MINB) cell_pipeline4_kernel(const Cell4Par
                 centre = block_median_smem<NT>(buf, my_fb, len, G, s1, s2, red, phase, cand, cand_n);
             }
         } else if (p.center == 2) {
+            const double S1 = warp_sum_d((lane < NW) ? red.d[phase][0][lane] : 0.0);
+            phase ^= 1;
             centre = S1 / (double)G;
         }
 
