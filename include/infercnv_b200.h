@@ -332,13 +332,19 @@ ICNV_API int icnv_debug_random_trees(double *out5);
  *   passes 1e-4 / 1e-4; jitter_sd = 0 keeps every tie and makes the statistic deterministic.
  * Y (G x C; may be X), p_raw and p_adj (G x (n_sub n_ref), column-major, column s * n_ref + j) are each nullable.
  * An empty group, an index out of range, an unknown test or rule code, jitter_sd < 0: ICNV_E_BAD_ARG; NaN / Inf in a listed
- * cell: ICNV_E_NONFINITE; not enough device memory: ICNV_E_NOMEM. */
+ * cell: ICNV_E_NONFINITE; not enough device memory: ICNV_E_NOMEM.
+ * Several device slots (icnv_init_devices): the genes are cut into one contiguous range per device, each device uploads only
+ * its genes of the listed columns (in sub-slabs sized from its free memory) and tests them; the p rows are gathered on the
+ * host, every device runs BH on all of them and masks its own range of cells, streamed through it in chunks.  The output
+ * bytes are those of one device, and X need not fit on any one of them. */
 ICNV_API int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t C, const int32_t *ref_off,
                                   const int32_t *ref_idx, int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub,
                                   int test, double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd,
                                   uint64_t seed, double *p_raw, double *p_adj);
 /* What the last mask call did: out7 = {gene tiles, genes per tile, ms of (a) gather, (b) reference sorts / group statistics,
- * (c) pair tests, (d) BH, (e) mask} (device time summed over the tiles); zeros before any call. */
+ * (c) pair tests, (d) BH, (e) mask} (device time summed over the tiles); zeros before any call.  With several device slots:
+ * the tiles summed over the devices, the largest tile, and each stage's time on the device where it took longest (the
+ * gather is the transposition of the uploaded columns; BH and the mask are summed over a device's cell chunks). */
 ICNV_API int icnv_debug_mask_non_de(double *out7);
 
 /* Gibbs sampling of inferCNVBayesNet (R/inferCNV_BayesNet.R run_gibb_sampling, :1054-1107; run() step 18) for n_reg CNV
@@ -585,6 +591,39 @@ ICNV_API int icnv_dev_mask_non_de_f64(const double *X, int64_t ldx, double *Y, i
                                       const int32_t *sub_off /*host*/, const int32_t *sub_idx /*host*/, int n_sub, int test,
                                       double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd,
                                       uint64_t seed, double *p_raw, double *p_adj, void *stream);
+/* The stages of icnv_dev_mask_non_de_f64 on their own, for a caller that splits the genes over devices or ranks (Engine.
+ * mask_non_de_sharded): each rank packs the listed cells it holds for every rank's gene range, the blocks are exchanged
+ * (all-to-all), each rank places what it received into slab rows and tests its genes, the p rows are all-gathered, and every
+ * rank runs BH on all of them and masks its own cells.  Every stage depends on a gene only through its absolute index and
+ * on a cell only through its global list position, so the bytes equal one device's for any split.
+ * icnv_dev_de_pack_f64: per destination d, the gene-major block out_d[gl * m + k] = X[gene_lo[d] + gl + ldx * d_cols[k]]
+ *   (gene_hi[d] - gene_lo[d] genes x m cells, d_cols on the device, each in [0, C)), the blocks back to back in destination
+ *   order; *err_flag |= 1 (device int) on a non-finite value.  Asynchronous on `stream`.
+ * icnv_dev_de_place_f64: R holds one gene-major block of n genes x src_m[q] cells per source q, back to back in source order;
+ *   d_tags (device, T entries in the same order) is each received cell's global list position (references in group order,
+ *   then the subclusters, as icnv_mask_non_de_f64 lists them).  Z[gl * T + d_tags[e]] = the value: the n x T slab rows.
+ *   sum(src_m) must be T.  Asynchronous on `stream`.
+ * icnv_dev_de_slab_tests_f64: stages (b) and (c) on the slab rows Z (n x T, gene-major) of the absolute genes g0 .. g0 + n:
+ *   p of pair s * n_ref + j and gene g0 + gl into p_raw[(s * n_ref + j) * ldp + gl].  Group sizes as the CSR offsets of
+ *   icnv_mask_non_de_f64 (HOST arrays; their total must be T).  Z must be finite (the pack or gather reports it).
+ *   Synchronises `stream`.
+ * icnv_dev_de_bh_mask_f64: BH of every pair over the whole p_raw (rows of G), into p_adj (nullable), then the mask of the C
+ *   columns of X into Y (nullable: BH only; may be X).  sub_size[s]: subcluster s's whole list length (the < 5 rule);
+ *   ref_idx / sub_off / sub_idx (HOST, 0-based columns of this block): its reference cells and, per subcluster, its cells
+ *   (possibly none).  Synchronises `stream`. */
+ICNV_API int icnv_dev_de_pack_f64(const double *X, int64_t ldx, const int32_t *d_cols, int64_t m, int n_dst,
+                                  const int64_t *gene_lo /*host*/, const int64_t *gene_hi /*host*/, double *out, int *err_flag,
+                                  void *stream);
+ICNV_API int icnv_dev_de_place_f64(const double *R, int64_t n, int n_src, const int64_t *src_m /*host*/, const int32_t *d_tags,
+                                   int64_t T, double *Z, void *stream);
+ICNV_API int icnv_dev_de_slab_tests_f64(const double *Z, int64_t T, int64_t g0, int64_t n, const int32_t *ref_off /*host*/,
+                                        int n_ref, const int32_t *sub_off /*host*/, int n_sub, int test, double jitter_mean,
+                                        double jitter_sd, uint64_t seed, double *p_raw, int64_t ldp, void *stream);
+ICNV_API int icnv_dev_de_bh_mask_f64(const double *p_raw, int64_t G, int n_ref, int n_sub, const int32_t *sub_size /*host*/,
+                                     double p_thresh, double *p_adj, const double *X, int64_t ldx, double *Y, int64_t ldy,
+                                     int64_t C, const int32_t *ref_idx /*host*/, int64_t n_ref_cells,
+                                     const int32_t *sub_off /*host*/, const int32_t *sub_idx /*host*/, int rule, double mask_val,
+                                     void *stream);
 /* icnv_bayesnet_f64 on device pointers: X (column stride ldx >= G), theta, state_counts, loglik (nullable); the region lists,
  * pooled, mu and tau are HOST arrays.  Synchronises `stream` after the log-likelihood pass (non-finite check) and at the end. */
 ICNV_API int icnv_dev_bayesnet_f64(const double *X, int64_t ldx, int64_t G, int64_t C, const int32_t *gene_off /*host*/,

@@ -68,6 +68,12 @@ SIGNATURES = {
     "icnv_dev_mask_non_de_f64": (c_int, [_P, c_i64, _P, c_i64, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,
                                          c_int, ct.c_double, ct.c_double, ct.c_double, ct.c_uint64, _P, _P, _P]),
     "icnv_debug_mask_non_de": (c_int, [_P]),
+    "icnv_dev_de_pack_f64": (c_int, [_P, c_i64, _P, c_i64, c_int, _P, _P, _P, _P, _P]),
+    "icnv_dev_de_place_f64": (c_int, [_P, c_i64, c_int, _P, _P, c_i64, _P, _P]),
+    "icnv_dev_de_slab_tests_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, c_int, _P, c_int, c_int, ct.c_double, ct.c_double,
+                                           ct.c_uint64, _P, c_i64, _P]),
+    "icnv_dev_de_bh_mask_f64": (c_int, [_P, c_i64, c_int, c_int, _P, ct.c_double, _P, _P, c_i64, _P, c_i64, c_i64, _P, c_i64,
+                                        _P, _P, c_int, ct.c_double, _P]),
     "icnv_bayesnet_f64": (c_int, [_P, c_i64, c_i64, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, ct.c_uint64,
                                   _P, _P, _P]),
     "icnv_dev_bayesnet_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int,

@@ -1975,6 +1975,25 @@ int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G,
                 double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd, unsigned long long seed,
                 double *p_raw, double *p_adj, void *stream, const char *who) __attribute__((weak));
 void de_mask_stats(double *out7) __attribute__((weak));
+void de_mask_set_stats(const double *in7) __attribute__((weak));
+int de_pack_dev(const double *X, int64_t ldx, const int32_t *d_cols, int64_t m, int n_dst, const int64_t *gene_lo,
+                const int64_t *gene_hi, double *out, int *flag, void *stream, const char *who) __attribute__((weak));
+int de_place_dev(const double *R, int64_t n, int n_src, const int64_t *src_m, const int32_t *d_tags, int64_t T, double *Z,
+                 void *stream, const char *who) __attribute__((weak));
+int de_slab_tests_dev(const double *Z, int64_t T, int64_t g0, int64_t n, const int32_t *ref_off, int n_ref,
+                      const int32_t *sub_off, int n_sub, int test, double jitter_mean, double jitter_sd,
+                      unsigned long long seed, double *p_raw, int64_t ldp, void *stream, double *times,
+                      const char *who) __attribute__((weak));
+int de_bh_mask_dev(const double *p_raw, int64_t G, int n_ref, int n_sub, const int32_t *sub_size, double p_thresh,
+                   double *p_adj, const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t C, const int32_t *ref_idx,
+                   int64_t n_ref_cells, const int32_t *sub_off, const int32_t *sub_idx, int rule, double mask_val,
+                   void *stream, double *times, const char *who) __attribute__((weak));
+// several device slots (icnv_de_multi.cu)
+int de_mask_multi(int n_dev, const double *X, double *Y, int64_t G, int64_t C, const int32_t *ref_off, const int32_t *ref_idx,
+                  int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub, int test, double p_thresh, int rule,
+                  double mask_val, double jitter_mean, double jitter_sd, uint64_t seed, double *p_raw,
+                  double *p_adj) __attribute__((weak));
+
 }  // namespace icnv
 
 extern "C" {
@@ -1995,6 +2014,11 @@ int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t C, const
     if (!icnv::de_mask_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_mask_non_de_f64: this build has no DE kernels");
     ICNV_HOST_PROLOGUE();
     if (!X || G <= 0 || C <= 0 || n_ref < 1 || n_sub < 0) return set_error(ICNV_E_BAD_ARG, "icnv_mask_non_de_f64: bad argument");
+    if (device_slots() > 1) {
+        if (!icnv::de_mask_multi) return set_error(ICNV_E_UNSUPPORTED, "icnv_mask_non_de_f64: this build has no multi-device DE path");
+        return icnv::de_mask_multi(device_slots(), X, Y, G, C, ref_off, ref_idx, n_ref, sub_off, sub_idx, n_sub, test, p_thresh, rule,
+                                   mask_val, jitter_mean, jitter_sd, seed, p_raw, p_adj);
+    }
     const int64_t npair = (int64_t)n_sub * n_ref;
     int rc;
     double *dX = nullptr;
@@ -2012,6 +2036,35 @@ int icnv_mask_non_de_f64(const double *X, double *Y, int64_t G, int64_t C, const
         ICNV_CUDA(cudaMemcpyAsync(p_adj, d_p + G * npair, sizeof(double) * (size_t)(G * npair), cudaMemcpyDeviceToHost, st));
     ICNV_CUDA(cudaStreamSynchronize(st));
     return ICNV_OK;
+}
+
+int icnv_dev_de_pack_f64(const double *X, int64_t ldx, const int32_t *d_cols, int64_t m, int n_dst, const int64_t *gene_lo,
+                         const int64_t *gene_hi, double *out, int *err_flag, void *stream) {
+    if (!icnv::de_pack_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_de_pack_f64: this build has no DE kernels");
+    return icnv::de_pack_dev(X, ldx, d_cols, m, n_dst, gene_lo, gene_hi, out, err_flag, stream, "icnv_dev_de_pack_f64");
+}
+
+int icnv_dev_de_place_f64(const double *R, int64_t n, int n_src, const int64_t *src_m, const int32_t *d_tags, int64_t T,
+                          double *Z, void *stream) {
+    if (!icnv::de_place_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_de_place_f64: this build has no DE kernels");
+    return icnv::de_place_dev(R, n, n_src, src_m, d_tags, T, Z, stream, "icnv_dev_de_place_f64");
+}
+
+int icnv_dev_de_slab_tests_f64(const double *Z, int64_t T, int64_t g0, int64_t n, const int32_t *ref_off, int n_ref,
+                               const int32_t *sub_off, int n_sub, int test, double jitter_mean, double jitter_sd, uint64_t seed,
+                               double *p_raw, int64_t ldp, void *stream) {
+    if (!icnv::de_slab_tests_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_de_slab_tests_f64: this build has no DE kernels");
+    return icnv::de_slab_tests_dev(Z, T, g0, n, ref_off, n_ref, sub_off, n_sub, test, jitter_mean, jitter_sd, seed, p_raw, ldp,
+                                   stream, nullptr, "icnv_dev_de_slab_tests_f64");
+}
+
+int icnv_dev_de_bh_mask_f64(const double *p_raw, int64_t G, int n_ref, int n_sub, const int32_t *sub_size, double p_thresh,
+                            double *p_adj, const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t C,
+                            const int32_t *ref_idx, int64_t n_ref_cells, const int32_t *sub_off, const int32_t *sub_idx,
+                            int rule, double mask_val, void *stream) {
+    if (!icnv::de_bh_mask_dev) return set_error(ICNV_E_UNSUPPORTED, "icnv_dev_de_bh_mask_f64: this build has no DE kernels");
+    return icnv::de_bh_mask_dev(p_raw, G, n_ref, n_sub, sub_size, p_thresh, p_adj, X, ldx, Y, ldy, C, ref_idx, n_ref_cells,
+                                sub_off, sub_idx, rule, mask_val, stream, nullptr, "icnv_dev_de_bh_mask_f64");
 }
 
 int icnv_debug_mask_non_de(double *out7) {

@@ -26,6 +26,11 @@
 // reference row by binary search - W and sum(t^3 - t) in exact integers - then p; after all tiles (d) BH per pair and (e)
 // one streaming pass per cell column.  Sorts are bitonic in shared memory up to SORT_SMEM bytes and in global scratch
 // beyond, as in icnv_random_trees.cu.
+//
+// The stages are also entry points of their own, for callers that split the genes over devices or ranks: the pack of a
+// rank's listed cells per destination gene range (the gather's transpose), the placing of received blocks by list position,
+// (b) + (c) on a slab of genes, and (d) + (e) on a block of cells.  A split gives the bytes of one call for any number of
+// parts (icnv_de_multi.cu, device.py's Engine.mask_non_de_sharded).
 #include "icnv_common.cuh"
 
 #include <algorithm>
@@ -184,9 +189,9 @@ __device__ double wilcox_p(long long u2, long long ties, int nx, int ny, const i
 
 // (c) Wilcoxon: per item (gene gl, pair) the subcluster's jittered row sorted; each run of equal values v (b of them) adds
 // b (2 lo + a) to 2 U_y and (a + b)^3 - (a + b) - (a^3 - a) to the ties, a = #(x == v), lo = #(x < v) in the sorted
-// reference row.  p into PR[pair G + g0 + gl].
+// reference row.  p into PR[pair ldp + gl] (g0 + gl the absolute gene).
 __global__ void __launch_bounds__(NT) pair_wilcox_kernel(const double *__restrict__ Z, int64_t T, int64_t gt, int64_t g0,
-                                                         int64_t G, const int32_t *__restrict__ ref_off,
+                                                         int64_t ldp, const int32_t *__restrict__ ref_off,
                                                          const int32_t *__restrict__ sub_off, int n_ref, int n_sub,
                                                          int64_t R_tot, unsigned long long seed, double jm, double js,
                                                          const double *__restrict__ RS, const long long *__restrict__ TS,
@@ -220,7 +225,7 @@ __global__ void __launch_bounds__(NT) pair_wilcox_kernel(const double *__restric
         ties = block_sum_ll(ties, red);
         if (threadIdx.x == 0) {
             const long long u2x = 2 * (long long)nx * ny - u2y;
-            PR[pair * G + g0 + gl] = wilcox_p(u2x, ties + TS[gl * n_ref + j], nx, ny, cdf_idx, cdf);
+            PR[pair * ldp + gl] = wilcox_p(u2x, ties + TS[gl * n_ref + j], nx, ny, cdf_idx, cdf);
         }
         __syncthreads();
     }
@@ -327,8 +332,8 @@ __device__ double t_two_sided(double t, double df) {
     return 1.0 - bt * betacf(b, a, y) / b;
 }
 
-// (c) t: per (pair, gene gl), one thread each.  t.test.default's arithmetic in its order.
-__global__ void __launch_bounds__(NT) pair_t_kernel(const double *__restrict__ ST, int64_t gt, int64_t g0, int64_t G,
+// (c) t: per (pair, gene gl), one thread each.  t.test.default's arithmetic in its order.  p into PR[pair ldp + gl].
+__global__ void __launch_bounds__(NT) pair_t_kernel(const double *__restrict__ ST, int64_t gt, int64_t ldp,
                                                     const int32_t *__restrict__ all_off, int n_ref, int n_sub, double *PR) {
     const int ng = n_ref + n_sub;
     const int64_t npair = (int64_t)n_sub * n_ref, items = gt * npair;
@@ -348,7 +353,7 @@ __global__ void __launch_bounds__(NT) pair_t_kernel(const double *__restrict__ S
             if (!(se < lim)) p = t_two_sided((mx - my) / se, df);   // se = 0 = lim: t and df NaN, so p NaN as in R
             if (se == 0.0 && !(se < lim)) p = __longlong_as_double(0x7ff8000000000000ll);
         }
-        PR[pair * G + g0 + gl] = p;
+        PR[pair * ldp + gl] = p;
     }
 }
 
@@ -418,6 +423,17 @@ __global__ void __launch_bounds__(NT) mask_kernel(const double *X, int64_t ldx, 
     }
 }
 
+// Receiving side of the gene exchange of the rank-sharded path: `blk` is one source rank's gene-major block (n genes x m
+// listed cells, in that rank's list order) and tags[k] the global list position of its entry k, so each value goes
+// straight to its place in the slab rows Z (n x T, every row in global list order).
+__global__ void __launch_bounds__(NT) place_kernel(const double *__restrict__ blk, int64_t n, int64_t m,
+                                                   const int32_t *__restrict__ tags, int64_t T, double *__restrict__ Z) {
+    for (int64_t i = (int64_t)blockIdx.x * NT + threadIdx.x; i < n * m; i += (int64_t)gridDim.x * NT) {
+        const int64_t gl = i / m, k = i - gl * m;
+        Z[gl * T + tags[k]] = blk[i];
+    }
+}
+
 }  // namespace de
 
 using namespace de;
@@ -449,6 +465,262 @@ static double g_de_stats[7];
 
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
+namespace {
+
+// one device allocation carved into 256-byte aligned pieces
+struct Layout {
+    size_t bytes = 0;
+    size_t take(size_t b) {
+        const size_t o = bytes;
+        bytes += align256(b);
+        return o;
+    }
+};
+
+// Host side of the tests (stages (b) and (c)) for one set of groups: every group's offsets over the T list positions
+// (reference groups, then subclusters), the exact null tables of the Wilcoxon pairs with both sizes < 50, the sort sizes.
+struct TestPlan {
+    int n_ref = 0, n_sub = 0, test = 0;
+    int64_t R_tot = 0, T = 0;
+    std::vector<int32_t> all_off, cdf_idx;
+    std::vector<double> cdf;
+    int Psort = 1;   // the largest row sort
+    bool sort_global = false;
+};
+
+int make_test_plan(const int32_t *ref_off, int n_ref, const int32_t *sub_off, int n_sub, int test, TestPlan &p,
+                   const char *who) {
+    if (n_ref < 1 || n_sub < 0 || !ref_off || (n_sub > 0 && !sub_off)) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    if (test != 0 && test != 1) return set_error(ICNV_E_BAD_ARG, "%s: unknown test code %d", who, test);
+    if (ref_off[0] != 0 || (n_sub > 0 && sub_off[0] != 0)) return set_error(ICNV_E_BAD_ARG, "%s: offsets must start at 0", who);
+    for (int k = 0; k < n_ref; ++k)
+        if (ref_off[k + 1] <= ref_off[k]) return set_error(ICNV_E_BAD_ARG, "%s: reference group %d is empty", who, k);
+    for (int k = 0; k < n_sub; ++k)
+        if (sub_off[k + 1] <= sub_off[k]) return set_error(ICNV_E_BAD_ARG, "%s: subcluster %d is empty", who, k);
+    p.n_ref = n_ref;
+    p.n_sub = n_sub;
+    p.test = test;
+    p.R_tot = ref_off[n_ref];
+    p.T = p.R_tot + (n_sub > 0 ? sub_off[n_sub] : 0);
+    if (p.T > (int64_t)INT32_MAX / 2) return set_error(ICNV_E_UNSUPPORTED, "%s: %lld listed cells", who, (long long)p.T);
+    p.all_off.assign((size_t)(n_ref + n_sub + 1), 0);
+    for (int k = 0; k <= n_ref; ++k) p.all_off[(size_t)k] = ref_off[k];
+    for (int k = 1; k <= n_sub; ++k) p.all_off[(size_t)(n_ref + k)] = (int32_t)(p.R_tot + sub_off[k]);
+    p.cdf_idx.assign((size_t)EXACT_N * EXACT_N, -1);
+    p.cdf.clear();
+    int max_ny = 1, max_nx = 1;
+    for (int j = 0; j < n_ref; ++j) max_nx = std::max(max_nx, ref_off[j + 1] - ref_off[j]);
+    for (int s = 0; s < n_sub; ++s) max_ny = std::max(max_ny, sub_off[s + 1] - sub_off[s]);
+    if (test == 0)
+        for (int s = 0; s < n_sub; ++s)
+            for (int j = 0; j < n_ref; ++j) {
+                const int nx = ref_off[j + 1] - ref_off[j], ny = sub_off[s + 1] - sub_off[s];
+                if (nx >= EXACT_N || ny >= EXACT_N || p.cdf_idx[(size_t)(nx * EXACT_N + ny)] >= 0) continue;
+                p.cdf_idx[(size_t)(nx * EXACT_N + ny)] = (int32_t)p.cdf.size();
+                rank_sum_cdf(nx, ny, p.cdf);
+            }
+    if (p.cdf.empty()) p.cdf.push_back(0.0);
+    p.Psort = 1;
+    while (p.Psort < std::max(max_nx, max_ny)) p.Psort <<= 1;
+    p.sort_global = sizeof(double) * (size_t)p.Psort > SORT_SMEM;
+    return ICNV_OK;
+}
+
+// Device side of a TestPlan: its tables and sort scratch (fixed) and the per-gene scratch of tiles of up to gt genes.
+struct TestDev {
+    size_t o_alloff = 0, o_cdfidx = 0, o_cdf = 0, o_sort = 0, o_rs = 0, o_ts = 0;
+    int32_t *alloff = nullptr, *cdfidx = nullptr;
+    double *cdf = nullptr, *sort = nullptr, *RS = nullptr, *ST = nullptr;
+    long long *TS = nullptr;
+    int grid_sort = 0;
+
+    void fixed(const TestPlan &p, int sm_count, Layout &L) {
+        grid_sort = sm_count * (p.sort_global ? 4 : 16);
+        o_alloff = L.take(sizeof(int32_t) * p.all_off.size());
+        o_cdfidx = L.take(sizeof(int32_t) * p.cdf_idx.size());
+        o_cdf = L.take(sizeof(double) * p.cdf.size());
+        o_sort = L.take(p.sort_global ? sizeof(double) * (size_t)p.Psort * grid_sort : 0);
+    }
+    static size_t per_gene(const TestPlan &p) {
+        return p.test == 0 ? sizeof(double) * (size_t)p.R_tot + sizeof(long long) * (size_t)p.n_ref
+                           : sizeof(double) * 2 * (size_t)(p.n_ref + p.n_sub);
+    }
+    void tiles(const TestPlan &p, int64_t gt, Layout &L) {
+        const int ng = p.n_ref + p.n_sub;
+        o_rs = L.take(p.test == 0 ? sizeof(double) * (size_t)(gt * p.R_tot) : 0);
+        o_ts = L.take(p.test == 0 ? sizeof(long long) * (size_t)(gt * p.n_ref) : sizeof(double) * 2 * (size_t)(gt * ng));
+    }
+    void bind(const TestPlan &p, char *buf) {
+        alloff = (int32_t *)(buf + o_alloff);
+        cdfidx = (int32_t *)(buf + o_cdfidx);
+        cdf = (double *)(buf + o_cdf);
+        sort = p.sort_global ? (double *)(buf + o_sort) : nullptr;
+        RS = (double *)(buf + o_rs);
+        TS = (long long *)(buf + o_ts);
+        ST = (double *)(buf + o_ts);
+    }
+    int upload(const TestPlan &p, cudaStream_t st) const {
+        ICNV_CUDA(cudaMemcpyAsync(alloff, p.all_off.data(), sizeof(int32_t) * p.all_off.size(), cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaMemcpyAsync(cdfidx, p.cdf_idx.data(), sizeof(int32_t) * p.cdf_idx.size(), cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaMemcpyAsync(cdf, p.cdf.data(), sizeof(double) * p.cdf.size(), cudaMemcpyHostToDevice, st));
+        const size_t smem_sort = p.sort_global ? 0 : sizeof(double) * (size_t)p.Psort;
+        if (smem_sort > 48 * 1024) {
+            ICNV_CUDA(cudaFuncSetAttribute(ref_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
+            ICNV_CUDA(cudaFuncSetAttribute(pair_wilcox_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
+        }
+        return ICNV_OK;
+    }
+    // stages (b) and (c) on the n gene-major rows Z (absolute genes g0 ..): p into PR[pair ldp + gl].  `mid`, when given,
+    // is recorded between the two stages.
+    int launch(const TestPlan &p, const double *Z, int64_t g0, int64_t n, double *PR, int64_t ldp, double jm, double js,
+               unsigned long long seed, int sm_count, cudaStream_t st, cudaEvent_t mid) const {
+        const int64_t npair = (int64_t)p.n_sub * p.n_ref;
+        const int ng = p.n_ref + p.n_sub;
+        const size_t smem_sort = p.sort_global ? 0 : sizeof(double) * (size_t)p.Psort;
+        const int32_t *refoff = alloff, *suboff = alloff + p.n_ref;   // list positions of every group within a Z row
+        if (p.test == 0) {
+            const unsigned gb = (unsigned)std::min<int64_t>(n * p.n_ref, grid_sort);
+            ref_sort_kernel<<<gb, NT, smem_sort, st>>>(Z, p.T, n, g0, refoff, p.n_ref, p.R_tot, seed, jm, js, RS, TS, sort,
+                                                       p.Psort);
+            ICNV_CHECK_LAUNCH("ref_sort_kernel");
+        } else {
+            const unsigned gb = (unsigned)std::min<int64_t>(n * ng, (int64_t)sm_count * 16);
+            group_stats_kernel<<<gb, NT, 0, st>>>(Z, p.T, n, alloff, ng, ST);
+            ICNV_CHECK_LAUNCH("group_stats_kernel");
+        }
+        if (mid) ICNV_CUDA(cudaEventRecord(mid, st));
+        if (npair > 0 && p.test == 0) {
+            const unsigned gb = (unsigned)std::min<int64_t>(n * npair, grid_sort);
+            pair_wilcox_kernel<<<gb, NT, smem_sort, st>>>(Z, p.T, n, g0, ldp, refoff, suboff, p.n_ref, p.n_sub, p.R_tot, seed,
+                                                          jm, js, RS, TS, cdfidx, cdf, PR, sort, p.Psort);
+            ICNV_CHECK_LAUNCH("pair_wilcox_kernel");
+        } else if (npair > 0) {
+            const unsigned gb = (unsigned)std::min<int64_t>((n * npair + NT - 1) / NT, (int64_t)sm_count * 32);
+            pair_t_kernel<<<gb, NT, 0, st>>>(ST, n, ldp, alloff, p.n_ref, p.n_sub, PR);
+            ICNV_CHECK_LAUNCH("pair_t_kernel");
+        }
+        return ICNV_OK;
+    }
+};
+
+// Host side of the mask (stage (e)) for a block of C columns: per cell the count's start (reference cells and the cells of a
+// tested subcluster of < 5 list entries start at n_ref) and the >= 5-entry subclusters holding it, each once.  sub_size[s]
+// is subcluster s's whole list length; sub_off / sub_idx list the cells of the block it holds (possibly none).
+struct MaskPlan {
+    std::vector<unsigned char> base;
+    std::vector<int32_t> cell_off, cell_sub;
+};
+
+int make_mask_plan(int64_t C, const int32_t *ref_idx, int64_t n_ref_cells, const int32_t *sub_off, const int32_t *sub_idx,
+                   int n_sub, const int32_t *sub_size, MaskPlan &m, const char *who) {
+    for (int64_t i = 0; i < n_ref_cells; ++i)
+        if (ref_idx[i] < 0 || ref_idx[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index %d out of range", who, ref_idx[i]);
+    for (int s = 0; s < n_sub; ++s)
+        for (int32_t i = sub_off[s]; i < sub_off[s + 1]; ++i)
+            if (sub_idx[i] < 0 || sub_idx[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index %d out of range", who, sub_idx[i]);
+    m.base.assign((size_t)C, 0);
+    for (int64_t i = 0; i < n_ref_cells; ++i) m.base[(size_t)ref_idx[i]] = 1;
+    std::vector<int32_t> last((size_t)C, -1);
+    m.cell_off.assign((size_t)C + 1, 0);
+    for (int s = 0; s < n_sub; ++s) {
+        const bool small = sub_size[s] < 5;
+        for (int32_t i = sub_off[s]; i < sub_off[s + 1]; ++i) {
+            const int32_t c = sub_idx[i];
+            if (small) m.base[(size_t)c] = 1;
+            else if (last[(size_t)c] != s) { last[(size_t)c] = s; m.cell_off[(size_t)c + 1]++; }
+        }
+    }
+    for (int64_t c = 0; c < C; ++c) m.cell_off[(size_t)c + 1] += m.cell_off[(size_t)c];
+    m.cell_sub.assign((size_t)std::max<int32_t>(m.cell_off[(size_t)C], 1), 0);
+    std::vector<int32_t> fill(m.cell_off.begin(), m.cell_off.end() - 1);
+    std::fill(last.begin(), last.end(), -1);
+    for (int s = 0; s < n_sub; ++s) {
+        if (sub_size[s] < 5) continue;
+        for (int32_t i = sub_off[s]; i < sub_off[s + 1]; ++i) {
+            const int32_t c = sub_idx[i];
+            if (last[(size_t)c] != s) { last[(size_t)c] = s; m.cell_sub[(size_t)fill[(size_t)c]++] = s; }
+        }
+    }
+    return ICNV_OK;
+}
+
+// Device side of stages (d) and (e): the DE bytes, BH's sort scratch and a MaskPlan's tables.
+struct BhMaskDev {
+    size_t o_de = 0, o_bhk = 0, o_bhi = 0, o_base = 0, o_celloff = 0, o_cellsub = 0;
+    unsigned char *DE = nullptr, *base = nullptr;
+    double *bhk = nullptr;
+    int32_t *bhi = nullptr, *celloff = nullptr, *cellsub = nullptr;
+    int PG = 1, grid_bh = 1;
+    bool bh_global = false;
+
+    void fixed(int64_t G, int64_t npair, const MaskPlan &m, int sm_count, Layout &L) {
+        PG = 1;
+        while (PG < G) PG <<= 1;
+        bh_global = (sizeof(double) + sizeof(int32_t)) * (size_t)PG > SORT_SMEM;
+        grid_bh = (int)std::min<int64_t>(std::max<int64_t>(npair, 1), (int64_t)sm_count * 2);
+        o_base = L.take(m.base.size());
+        o_celloff = L.take(sizeof(int32_t) * m.cell_off.size());
+        o_cellsub = L.take(sizeof(int32_t) * m.cell_sub.size());
+        o_de = L.take((size_t)(G * std::max<int64_t>(npair, 1)));
+        o_bhk = L.take(bh_global ? sizeof(double) * (size_t)PG * grid_bh : 0);
+        o_bhi = L.take(bh_global ? sizeof(int32_t) * (size_t)PG * grid_bh : 0);
+    }
+    void bind(char *buf) {
+        DE = (unsigned char *)(buf + o_de);
+        base = (unsigned char *)(buf + o_base);
+        celloff = (int32_t *)(buf + o_celloff);
+        cellsub = (int32_t *)(buf + o_cellsub);
+        bhk = bh_global ? (double *)(buf + o_bhk) : nullptr;
+        bhi = bh_global ? (int32_t *)(buf + o_bhi) : nullptr;
+    }
+    int upload(const MaskPlan &m, cudaStream_t st) const {
+        ICNV_CUDA(cudaMemcpyAsync(base, m.base.data(), m.base.size(), cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaMemcpyAsync(celloff, m.cell_off.data(), sizeof(int32_t) * m.cell_off.size(), cudaMemcpyHostToDevice, st));
+        ICNV_CUDA(cudaMemcpyAsync(cellsub, m.cell_sub.data(), sizeof(int32_t) * m.cell_sub.size(), cudaMemcpyHostToDevice, st));
+        return ICNV_OK;
+    }
+    int bh(const double *PR, int64_t G, int64_t npair, double thr, double *PA, cudaStream_t st) const {
+        if (npair == 0) return ICNV_OK;
+        const size_t smem_bh = bh_global ? 0 : (sizeof(double) + sizeof(int32_t)) * (size_t)PG;
+        if (smem_bh > 48 * 1024) ICNV_CUDA(cudaFuncSetAttribute(bh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bh));
+        bh_kernel<<<(unsigned)grid_bh, NT, smem_bh, st>>>(PR, G, npair, thr, PA, DE, bhk, bhi, PG);
+        ICNV_CHECK_LAUNCH("bh_kernel");
+        return ICNV_OK;
+    }
+    int mask(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C, int n_ref, int rule, double mask_val,
+             cudaStream_t st) const {
+        if (!Y || C == 0) return ICNV_OK;
+        mask_kernel<<<(unsigned)std::min<int64_t>(C, 65535), NT, 0, st>>>(X, ldx, Y, ldy, G, C, base, celloff, cellsub, n_ref,
+                                                                           DE, rule, mask_val);
+        ICNV_CHECK_LAUNCH("mask_kernel");
+        return ICNV_OK;
+    }
+};
+
+// free device memory less a 512 MB margin
+size_t usable_device_bytes() {
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) return 0;
+    return free_b > (size_t)(512 << 20) ? free_b - (size_t)(512 << 20) : 0;
+}
+
+int alloc_layout(char **buf, const Layout &L, cudaStream_t st, const char *who) {
+    if (cudaMallocAsync((void **)buf, L.bytes, st) != cudaSuccess) {
+        cudaGetLastError();
+        *buf = nullptr;
+        return set_error(ICNV_E_NOMEM, "%s: no room for %lld bytes", who, (long long)L.bytes);
+    }
+    return ICNV_OK;
+}
+
+int check_jitter(double jitter_mean, double jitter_sd, double p_thresh, const char *who) {
+    if (!std::isfinite(jitter_mean) || !std::isfinite(jitter_sd) || jitter_sd < 0.0 || std::isnan(p_thresh))
+        return set_error(ICNV_E_BAD_ARG, "%s: bad jitter or threshold", who);
+    return ICNV_OK;
+}
+
+}  // namespace
+
 int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G, int64_t C, const int32_t *ref_off,
                 const int32_t *ref_idx, int n_ref, const int32_t *sub_off, const int32_t *sub_idx, int n_sub, int test,
                 double p_thresh, int rule, double mask_val, double jitter_mean, double jitter_sd, unsigned long long seed,
@@ -459,157 +731,62 @@ int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G,
         return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
     if (test != 0 && test != 1) return set_error(ICNV_E_BAD_ARG, "%s: unknown test code %d", who, test);
     if (rule < 0 || rule > 2) return set_error(ICNV_E_BAD_ARG, "%s: unknown rule code %d", who, rule);
-    if (!std::isfinite(jitter_mean) || !std::isfinite(jitter_sd) || jitter_sd < 0.0 || std::isnan(p_thresh))
-        return set_error(ICNV_E_BAD_ARG, "%s: bad jitter or threshold", who);
-    if (ref_off[0] != 0 || (n_sub > 0 && sub_off[0] != 0)) return set_error(ICNV_E_BAD_ARG, "%s: offsets must start at 0", who);
-    for (int k = 0; k < n_ref; ++k)
-        if (ref_off[k + 1] <= ref_off[k]) return set_error(ICNV_E_BAD_ARG, "%s: reference group %d is empty", who, k);
-    for (int k = 0; k < n_sub; ++k)
-        if (sub_off[k + 1] <= sub_off[k]) return set_error(ICNV_E_BAD_ARG, "%s: subcluster %d is empty", who, k);
-    const int64_t R_tot = ref_off[n_ref], S_tot = n_sub > 0 ? sub_off[n_sub] : 0, T = R_tot + S_tot;
-    if (T > (int64_t)INT32_MAX / 2) return set_error(ICNV_E_UNSUPPORTED, "%s: %lld listed cells", who, (long long)T);
+    int rc = check_jitter(jitter_mean, jitter_sd, p_thresh, who);
+    if (rc) return rc;
+    TestPlan tp;
+    if ((rc = make_test_plan(ref_off, n_ref, sub_off, n_sub, test, tp, who))) return rc;
+    const int64_t R_tot = tp.R_tot, T = tp.T;
     std::vector<int32_t> cols((size_t)T);
     for (int64_t i = 0; i < R_tot; ++i) cols[(size_t)i] = ref_idx[i];
-    for (int64_t i = 0; i < S_tot; ++i) cols[(size_t)(R_tot + i)] = sub_idx[i];
+    for (int64_t i = R_tot; i < T; ++i) cols[(size_t)i] = sub_idx[i - R_tot];
     for (int32_t v : cols)
         if (v < 0 || v >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index %d out of range", who, v);
-    // every group's offsets over the T list positions: reference groups, then subclusters
-    std::vector<int32_t> all_off((size_t)(n_ref + n_sub + 1));
-    for (int k = 0; k <= n_ref; ++k) all_off[(size_t)k] = ref_off[k];
-    for (int k = 1; k <= n_sub; ++k) all_off[(size_t)(n_ref + k)] = (int32_t)(R_tot + sub_off[k]);
-    // the count's start per cell and, per cell, the >= 5-entry subclusters holding it (each once)
-    std::vector<unsigned char> base((size_t)C, 0);
-    for (int64_t i = 0; i < R_tot; ++i) base[(size_t)ref_idx[i]] = 1;
-    std::vector<int32_t> cnt((size_t)C + 1, 0), last((size_t)C, -1);
-    for (int s = 0; s < n_sub; ++s) {
-        const bool small = sub_off[s + 1] - sub_off[s] < 5;
-        for (int32_t i = sub_off[s]; i < sub_off[s + 1]; ++i) {
-            const int32_t c = sub_idx[i];
-            if (small) base[(size_t)c] = 1;
-            else if (last[(size_t)c] != s) { last[(size_t)c] = s; cnt[(size_t)c + 1]++; }
-        }
-    }
-    for (int64_t c = 0; c < C; ++c) cnt[(size_t)c + 1] += cnt[(size_t)c];
-    std::vector<int32_t> cell_sub((size_t)std::max<int32_t>(cnt[(size_t)C], 1)), fill(cnt.begin(), cnt.end() - 1);
-    std::fill(last.begin(), last.end(), -1);
-    for (int s = 0; s < n_sub; ++s) {
-        if (sub_off[s + 1] - sub_off[s] < 5) continue;
-        for (int32_t i = sub_off[s]; i < sub_off[s + 1]; ++i) {
-            const int32_t c = sub_idx[i];
-            if (last[(size_t)c] != s) { last[(size_t)c] = s; cell_sub[(size_t)fill[(size_t)c]++] = s; }
-        }
-    }
-    // exact null tables of the pairs with both sizes < 50 (Wilcoxon)
-    std::vector<int32_t> cdf_idx((size_t)EXACT_N * EXACT_N, -1);
-    std::vector<double> cdf;
-    int max_ny = 1, max_nx = 1;
-    for (int j = 0; j < n_ref; ++j) max_nx = std::max(max_nx, ref_off[j + 1] - ref_off[j]);
-    for (int s = 0; s < n_sub; ++s) max_ny = std::max(max_ny, sub_off[s + 1] - sub_off[s]);
-    if (test == 0)
-        for (int s = 0; s < n_sub; ++s)
-            for (int j = 0; j < n_ref; ++j) {
-                const int nx = ref_off[j + 1] - ref_off[j], ny = sub_off[s + 1] - sub_off[s];
-                if (nx >= EXACT_N || ny >= EXACT_N || cdf_idx[(size_t)(nx * EXACT_N + ny)] >= 0) continue;
-                cdf_idx[(size_t)(nx * EXACT_N + ny)] = (int32_t)cdf.size();
-                rank_sum_cdf(nx, ny, cdf);
-            }
-    if (cdf.empty()) cdf.push_back(0.0);
+    std::vector<int32_t> sub_size((size_t)std::max(n_sub, 1));
+    for (int s = 0; s < n_sub; ++s) sub_size[(size_t)s] = sub_off[s + 1] - sub_off[s];
+    MaskPlan mp;
+    if ((rc = make_mask_plan(C, ref_idx, R_tot, sub_off, sub_idx, n_sub, sub_size.data(), mp, who))) return rc;
 
     Ctx &c = ctx();
     cudaStream_t st = pick_stream(stream);
     const int64_t npair = (int64_t)n_sub * n_ref;
-    const int ng = n_ref + n_sub;
-    int Psort = 1;   // the largest row sort
-    while (Psort < std::max(max_nx, max_ny)) Psort <<= 1;
-    int PG = 1;
-    while (PG < G) PG <<= 1;
-    const bool sort_global = sizeof(double) * (size_t)Psort > SORT_SMEM;
-    const bool bh_global = (sizeof(double) + sizeof(int32_t)) * (size_t)PG > SORT_SMEM;
-    const int grid_sort = c.sm_count * (sort_global ? 4 : 16);
-    const int grid_bh = (int)std::min<int64_t>(std::max<int64_t>(npair, 1), (int64_t)c.sm_count * 2);
     // fixed part of the one device allocation
-    size_t fixed = 0;
-    auto take = [&](size_t b) { const size_t o = fixed; fixed += align256(b); return o; };
-    const size_t o_cols = take(sizeof(int32_t) * (size_t)T), o_alloff = take(sizeof(int32_t) * all_off.size()),
-                 o_base = take((size_t)C), o_celloff = take(sizeof(int32_t) * cnt.size()),
-                 o_cellsub = take(sizeof(int32_t) * cell_sub.size()), o_cdfidx = take(sizeof(int32_t) * cdf_idx.size()),
-                 o_cdf = take(sizeof(double) * cdf.size()), o_flag = take(sizeof(int)),
-                 o_pr = p_raw ? 0 : take(sizeof(double) * (size_t)(G * std::max<int64_t>(npair, 1))),
-                 o_pa = p_adj ? 0 : take(sizeof(double) * (size_t)(G * std::max<int64_t>(npair, 1))),
-                 o_de = take((size_t)(G * std::max<int64_t>(npair, 1))),
-                 o_sort = take(sort_global ? sizeof(double) * (size_t)Psort * grid_sort : 0),
-                 o_bhk = take(bh_global ? sizeof(double) * (size_t)PG * grid_bh : 0),
-                 o_bhi = take(bh_global ? sizeof(int32_t) * (size_t)PG * grid_bh : 0);
-    const size_t per_gene = sizeof(double) * (size_t)(T + (test == 0 ? R_tot : 0)) +
-                            (test == 0 ? sizeof(long long) * (size_t)n_ref : sizeof(double) * 2 * (size_t)ng);
-    size_t free_b = 0, total_b = 0;
-    ICNV_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    const size_t usable = free_b > (size_t)(512 << 20) ? free_b - (size_t)(512 << 20) : 0;
-    if (usable < fixed + per_gene + 4096) return set_error(ICNV_E_NOMEM, "%s: not even one gene fits in device memory", who);
-    const int64_t gt = std::min<int64_t>(G, (int64_t)((usable - fixed - 4096) / per_gene));
-    const size_t o_z = take(sizeof(double) * (size_t)(gt * T)), o_rs = take(test == 0 ? sizeof(double) * (size_t)(gt * R_tot) : 0),
-                 o_ts = take(test == 0 ? sizeof(long long) * (size_t)(gt * n_ref) : sizeof(double) * 2 * (size_t)(gt * ng));
+    Layout L;
+    TestDev td;
+    BhMaskDev bm;
+    const size_t o_cols = L.take(sizeof(int32_t) * (size_t)T), o_flag = L.take(sizeof(int)),
+                 o_pr = p_raw ? 0 : L.take(sizeof(double) * (size_t)(G * std::max<int64_t>(npair, 1))),
+                 o_pa = p_adj ? 0 : L.take(sizeof(double) * (size_t)(G * std::max<int64_t>(npair, 1)));
+    td.fixed(tp, c.sm_count, L);
+    bm.fixed(G, npair, mp, c.sm_count, L);
+    const size_t per_gene = sizeof(double) * (size_t)T + TestDev::per_gene(tp);
+    const size_t usable = usable_device_bytes();
+    if (usable < L.bytes + per_gene + 4096) return set_error(ICNV_E_NOMEM, "%s: not even one gene fits in device memory", who);
+    const int64_t gt = std::min<int64_t>(G, (int64_t)((usable - L.bytes - 4096) / per_gene));
+    const size_t o_z = L.take(sizeof(double) * (size_t)(gt * T));
+    td.tiles(tp, gt, L);
     char *buf = nullptr;
-    if (cudaMallocAsync((void **)&buf, fixed, st) != cudaSuccess) {
-        cudaGetLastError();
-        return set_error(ICNV_E_NOMEM, "%s: no room for %lld bytes", who, (long long)fixed);
-    }
-    int32_t *d_cols = (int32_t *)(buf + o_cols), *d_alloff = (int32_t *)(buf + o_alloff), *d_celloff = (int32_t *)(buf + o_celloff),
-            *d_cellsub = (int32_t *)(buf + o_cellsub), *d_cdfidx = (int32_t *)(buf + o_cdfidx);
-    unsigned char *d_base = (unsigned char *)(buf + o_base), *d_de = (unsigned char *)(buf + o_de);
-    double *d_cdf = (double *)(buf + o_cdf), *PR = p_raw ? p_raw : (double *)(buf + o_pr), *PA = p_adj ? p_adj : (double *)(buf + o_pa);
-    double *d_sort = sort_global ? (double *)(buf + o_sort) : nullptr, *d_bhk = bh_global ? (double *)(buf + o_bhk) : nullptr;
-    int32_t *d_bhi = bh_global ? (int32_t *)(buf + o_bhi) : nullptr;
+    if ((rc = alloc_layout(&buf, L, st, who))) return rc;
+    td.bind(tp, buf);
+    bm.bind(buf);
+    int32_t *d_cols = (int32_t *)(buf + o_cols);
     int *d_flag = (int *)(buf + o_flag);
-    double *Z = (double *)(buf + o_z), *RS = (double *)(buf + o_rs);
-    long long *TS = (long long *)(buf + o_ts);
-    double *ST = (double *)(buf + o_ts);
-    const int32_t *d_refoff = d_alloff, *d_suboff = d_alloff + n_ref;   // list positions of every group within a Z row
+    double *PR = p_raw ? p_raw : (double *)(buf + o_pr), *PA = p_adj ? p_adj : (double *)(buf + o_pa);
+    double *Z = (double *)(buf + o_z);
     cudaEvent_t ev[6] = {};
     for (auto &e : ev) ICNV_CUDA(cudaEventCreate(&e));
     auto body = [&]() -> int {
+        int rc2;
         ICNV_CUDA(cudaMemcpyAsync(d_cols, cols.data(), sizeof(int32_t) * (size_t)T, cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_alloff, all_off.data(), sizeof(int32_t) * all_off.size(), cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_base, base.data(), (size_t)C, cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_celloff, cnt.data(), sizeof(int32_t) * cnt.size(), cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_cellsub, cell_sub.data(), sizeof(int32_t) * cell_sub.size(), cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_cdfidx, cdf_idx.data(), sizeof(int32_t) * cdf_idx.size(), cudaMemcpyHostToDevice, st));
-        ICNV_CUDA(cudaMemcpyAsync(d_cdf, cdf.data(), sizeof(double) * cdf.size(), cudaMemcpyHostToDevice, st));
+        if ((rc2 = td.upload(tp, st)) || (rc2 = bm.upload(mp, st))) return rc2;
         ICNV_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
         double t[5] = {0, 0, 0, 0, 0};
-        const size_t smem_sort = sort_global ? 0 : sizeof(double) * (size_t)Psort;
-        if (smem_sort > 48 * 1024) {
-            ICNV_CUDA(cudaFuncSetAttribute(ref_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
-            ICNV_CUDA(cudaFuncSetAttribute(pair_wilcox_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
-        }
         for (int64_t g0 = 0; g0 < G; g0 += gt) {
             const int64_t n = std::min<int64_t>(gt, G - g0);
             ICNV_CUDA(cudaEventRecord(ev[0], st));
             gather_kernel<<<dim3((unsigned)((T + 31) / 32), (unsigned)((n + 31) / 32)), NT, 0, st>>>(X, ldx, d_cols, T, g0, n, Z, d_flag);
             ICNV_CHECK_LAUNCH("gather_kernel");
             ICNV_CUDA(cudaEventRecord(ev[1], st));
-            if (test == 0) {
-                const unsigned gb = (unsigned)std::min<int64_t>(n * n_ref, grid_sort);
-                ref_sort_kernel<<<gb, NT, smem_sort, st>>>(Z, T, n, g0, d_refoff, n_ref, R_tot, seed, jitter_mean, jitter_sd, RS,
-                                                           TS, d_sort, Psort);
-                ICNV_CHECK_LAUNCH("ref_sort_kernel");
-            } else {
-                const unsigned gb = (unsigned)std::min<int64_t>(n * ng, (int64_t)c.sm_count * 16);
-                group_stats_kernel<<<gb, NT, 0, st>>>(Z, T, n, d_alloff, ng, ST);
-                ICNV_CHECK_LAUNCH("group_stats_kernel");
-            }
-            ICNV_CUDA(cudaEventRecord(ev[2], st));
-            if (npair > 0 && test == 0) {
-                const unsigned gb = (unsigned)std::min<int64_t>(n * npair, grid_sort);
-                pair_wilcox_kernel<<<gb, NT, smem_sort, st>>>(Z, T, n, g0, G, d_refoff, d_suboff, n_ref, n_sub, R_tot,
-                                                              seed, jitter_mean, jitter_sd, RS, TS, d_cdfidx, d_cdf, PR,
-                                                              d_sort, Psort);
-                ICNV_CHECK_LAUNCH("pair_wilcox_kernel");
-            } else if (npair > 0) {
-                const unsigned gb = (unsigned)std::min<int64_t>((n * npair + NT - 1) / NT, (int64_t)c.sm_count * 32);
-                pair_t_kernel<<<gb, NT, 0, st>>>(ST, n, g0, G, d_alloff, n_ref, n_sub, PR);
-                ICNV_CHECK_LAUNCH("pair_t_kernel");
-            }
+            if ((rc2 = td.launch(tp, Z, g0, n, PR + g0, G, jitter_mean, jitter_sd, seed, c.sm_count, st, ev[2]))) return rc2;
             ICNV_CUDA(cudaEventRecord(ev[3], st));
             int h = 0;   // each tile's gather reports its own non-finite values
             ICNV_CUDA(cudaMemcpyAsync(&h, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -622,18 +799,9 @@ int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G,
             }
         }
         ICNV_CUDA(cudaEventRecord(ev[3], st));
-        if (npair > 0) {
-            const size_t smem_bh = bh_global ? 0 : (sizeof(double) + sizeof(int32_t)) * (size_t)PG;
-            if (smem_bh > 48 * 1024) ICNV_CUDA(cudaFuncSetAttribute(bh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bh));
-            bh_kernel<<<(unsigned)grid_bh, NT, smem_bh, st>>>(PR, G, npair, p_thresh, PA, d_de, d_bhk, d_bhi, PG);
-            ICNV_CHECK_LAUNCH("bh_kernel");
-        }
+        if ((rc2 = bm.bh(PR, G, npair, p_thresh, PA, st))) return rc2;
         ICNV_CUDA(cudaEventRecord(ev[4], st));
-        if (Y) {
-            mask_kernel<<<(unsigned)std::min<int64_t>(C, 65535), NT, 0, st>>>(X, ldx, Y, ldy, G, C, d_base, d_celloff, d_cellsub,
-                                                                               n_ref, d_de, rule, mask_val);
-            ICNV_CHECK_LAUNCH("mask_kernel");
-        }
+        if ((rc2 = bm.mask(X, ldx, Y, ldy, G, C, n_ref, rule, mask_val, st))) return rc2;
         ICNV_CUDA(cudaEventRecord(ev[5], st));
         ICNV_CUDA(cudaStreamSynchronize(st));
         float ms = 0.0f;
@@ -646,7 +814,7 @@ int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G,
         for (int s = 0; s < 5; ++s) g_de_stats[2 + s] = t[s];
         return ICNV_OK;
     };
-    const int rc = body();
+    rc = body();
     cudaFreeAsync(buf, st);
     for (auto &e : ev)
         if (e) cudaEventDestroy(e);
@@ -655,6 +823,179 @@ int de_mask_dev(const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t G,
 
 void de_mask_stats(double *out7) {
     for (int i = 0; i < 7; ++i) out7[i] = g_de_stats[i];
+}
+void de_mask_set_stats(const double *in7) {
+    for (int i = 0; i < 7; ++i) g_de_stats[i] = in7[i];
+}
+
+// ---- the stages on their own, for callers that split the genes over devices or ranks ----------------------------------
+
+// Stage (a) for an exchange: per destination d, the gene-major block (gene_hi[d] - gene_lo[d] genes x m listed cells) of
+// X's columns d_cols, blocks back to back in destination order - the same 32 x 32 transpose as the gather.
+int de_pack_dev(const double *X, int64_t ldx, const int32_t *d_cols, int64_t m, int n_dst, const int64_t *gene_lo,
+                const int64_t *gene_hi, double *out, int *flag, void *stream, const char *who) {
+    ICNV_REQUIRE_READY();
+    if (m < 0 || n_dst < 1 || !gene_lo || !gene_hi) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    int64_t total = 0;
+    for (int d = 0; d < n_dst; ++d) {
+        if (gene_lo[d] < 0 || gene_hi[d] < gene_lo[d] || gene_hi[d] > ldx)
+            return set_error(ICNV_E_BAD_ARG, "%s: gene range %d is [%lld, %lld)", who, d, (long long)gene_lo[d], (long long)gene_hi[d]);
+        total += gene_hi[d] - gene_lo[d];
+    }
+    if (m == 0 || total == 0) return ICNV_OK;
+    if (!X || !d_cols || !out || !flag) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    cudaStream_t st = pick_stream(stream);
+    double *o = out;
+    for (int d = 0; d < n_dst; ++d) {
+        const int64_t n = gene_hi[d] - gene_lo[d];
+        if (n == 0) continue;
+        gather_kernel<<<dim3((unsigned)((m + 31) / 32), (unsigned)((n + 31) / 32)), NT, 0, st>>>(X, ldx, d_cols, m, gene_lo[d], n,
+                                                                                                o, flag);
+        ICNV_CHECK_LAUNCH("gather_kernel");
+        o += n * m;
+    }
+    return ICNV_OK;
+}
+
+// The receiving side: R holds one block (n genes x src_m[q] cells) per source q, back to back in source order; d_tags the
+// global list positions of the received entries in the same order.  Fills the n x T slab rows Z.
+int de_place_dev(const double *R, int64_t n, int n_src, const int64_t *src_m, const int32_t *d_tags, int64_t T, double *Z,
+                 void *stream, const char *who) {
+    ICNV_REQUIRE_READY();
+    if (n < 0 || n_src < 1 || !src_m || T < 0) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    int64_t tot = 0;
+    for (int q = 0; q < n_src; ++q) {
+        if (src_m[q] < 0) return set_error(ICNV_E_BAD_ARG, "%s: source %d sends %lld cells", who, q, (long long)src_m[q]);
+        tot += src_m[q];
+    }
+    if (tot != T) return set_error(ICNV_E_BAD_ARG, "%s: the sources send %lld cells, the rows hold %lld", who, (long long)tot, (long long)T);
+    if (n == 0 || T == 0) return ICNV_OK;
+    if (!R || !d_tags || !Z) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    Ctx &c = ctx();
+    cudaStream_t st = pick_stream(stream);
+    int64_t e0 = 0;
+    for (int q = 0; q < n_src; ++q) {
+        const int64_t m = src_m[q];
+        if (m > 0) {
+            const unsigned gb = (unsigned)std::min<int64_t>((n * m + NT - 1) / NT, (int64_t)c.sm_count * 16);
+            place_kernel<<<gb, NT, 0, st>>>(R + n * e0, n, m, d_tags + e0, T, Z);
+            ICNV_CHECK_LAUNCH("place_kernel");
+        }
+        e0 += m;
+    }
+    return ICNV_OK;
+}
+
+// Stages (b) and (c) on the slab rows Z (n genes x T listed cells, gene-major, global list order) of absolute genes g0 ..:
+// p into p_raw[pair ldp + gl].  The per-gene scratch is tiled from free memory.  `times`, when given, gets the device ms of
+// (b) and (c) added.
+int de_slab_tests_dev(const double *Z, int64_t T, int64_t g0, int64_t n, const int32_t *ref_off, int n_ref,
+                      const int32_t *sub_off, int n_sub, int test, double jitter_mean, double jitter_sd,
+                      unsigned long long seed, double *p_raw, int64_t ldp, void *stream, double *times, const char *who) {
+    ICNV_REQUIRE_READY();
+    if (n < 0 || g0 < 0 || T < 1) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    int rc = check_jitter(jitter_mean, jitter_sd, 0.0, who);
+    if (rc) return rc;
+    TestPlan tp;
+    if ((rc = make_test_plan(ref_off, n_ref, sub_off, n_sub, test, tp, who))) return rc;
+    if (tp.T != T) return set_error(ICNV_E_BAD_ARG, "%s: the groups list %lld cells, the rows hold %lld", who, (long long)tp.T, (long long)T);
+    if (n == 0 || n_sub == 0) return ICNV_OK;   // no pair: nothing to write
+    if (!Z || !p_raw || ldp < n) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    Ctx &c = ctx();
+    cudaStream_t st = pick_stream(stream);
+    Layout L;
+    TestDev td;
+    td.fixed(tp, c.sm_count, L);
+    const size_t per_gene = TestDev::per_gene(tp), usable = usable_device_bytes();
+    if (usable < L.bytes + per_gene + 4096) return set_error(ICNV_E_NOMEM, "%s: not even one gene fits in device memory", who);
+    const int64_t gt = std::min<int64_t>(n, (int64_t)((usable - L.bytes - 4096) / per_gene));
+    td.tiles(tp, gt, L);
+    char *buf = nullptr;
+    if ((rc = alloc_layout(&buf, L, st, who))) return rc;
+    td.bind(tp, buf);
+    cudaEvent_t ev[3] = {};
+    for (auto &e : ev) ICNV_CUDA(cudaEventCreate(&e));
+    auto body = [&]() -> int {
+        int rc2;
+        if ((rc2 = td.upload(tp, st))) return rc2;
+        for (int64_t a = 0; a < n; a += gt) {
+            const int64_t nn = std::min<int64_t>(gt, n - a);
+            ICNV_CUDA(cudaEventRecord(ev[0], st));
+            if ((rc2 = td.launch(tp, Z + a * T, g0 + a, nn, p_raw + a, ldp, jitter_mean, jitter_sd, seed, c.sm_count, st, ev[1])))
+                return rc2;
+            ICNV_CUDA(cudaEventRecord(ev[2], st));
+            ICNV_CUDA(cudaStreamSynchronize(st));
+            float ms = 0.0f;
+            for (int s = 0; s < 2 && times; ++s) {
+                ICNV_CUDA(cudaEventElapsedTime(&ms, ev[s], ev[s + 1]));
+                times[s] += ms;
+            }
+        }
+        return ICNV_OK;
+    };
+    rc = body();
+    cudaFreeAsync(buf, st);
+    for (auto &e : ev)
+        if (e) cudaEventDestroy(e);
+    return rc;
+}
+
+// Stages (d) and (e): BH of the whole p_raw (G x n_pairs, pair rows of G), then the mask of a block of C columns of X
+// (nullable Y: BH only).  ref_idx: the block's reference cells; sub_off / sub_idx: per subcluster the block's cells of it
+// (possibly none), sub_size its whole list length.  `times`, when given, gets the device ms of (d) and (e).
+int de_bh_mask_dev(const double *p_raw, int64_t G, int n_ref, int n_sub, const int32_t *sub_size, double p_thresh,
+                   double *p_adj, const double *X, int64_t ldx, double *Y, int64_t ldy, int64_t C, const int32_t *ref_idx,
+                   int64_t n_ref_cells, const int32_t *sub_off, const int32_t *sub_idx, int rule, double mask_val,
+                   void *stream, double *times, const char *who) {
+    ICNV_REQUIRE_READY();
+    const int64_t npair = (int64_t)std::max(n_sub, 0) * n_ref;
+    if (G < 1 || n_ref < 1 || n_sub < 0 || C < 0 || n_ref_cells < 0 || (npair > 0 && (!p_raw || !sub_size)) ||
+        (n_ref_cells > 0 && !ref_idx) || (n_sub > 0 && (!sub_off || !sub_idx)) ||
+        (Y && C > 0 && (!X || ldx < G || ldy < G)))
+        return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    if (rule < 0 || rule > 2) return set_error(ICNV_E_BAD_ARG, "%s: unknown rule code %d", who, rule);
+    if (std::isnan(p_thresh)) return set_error(ICNV_E_BAD_ARG, "%s: bad threshold", who);
+    for (int s = 0; s < n_sub; ++s) {
+        if (sub_size[s] < 1) return set_error(ICNV_E_BAD_ARG, "%s: subcluster %d is empty", who, s);
+        if (sub_off[s + 1] < sub_off[s]) return set_error(ICNV_E_BAD_ARG, "%s: offsets of subcluster %d decrease", who, s);
+    }
+    if (n_sub > 0 && sub_off[0] != 0) return set_error(ICNV_E_BAD_ARG, "%s: offsets must start at 0", who);
+    MaskPlan mp;
+    int rc = make_mask_plan(Y ? C : 0, ref_idx, Y ? n_ref_cells : 0, sub_off, sub_idx, Y ? n_sub : 0, sub_size, mp, who);
+    if (rc) return rc;
+    Ctx &c = ctx();
+    cudaStream_t st = pick_stream(stream);
+    Layout L;
+    BhMaskDev bm;
+    const size_t o_pa = p_adj ? 0 : L.take(sizeof(double) * (size_t)(G * std::max<int64_t>(npair, 1)));
+    bm.fixed(G, npair, mp, c.sm_count, L);
+    char *buf = nullptr;
+    if ((rc = alloc_layout(&buf, L, st, who))) return rc;
+    bm.bind(buf);
+    double *PA = p_adj ? p_adj : (double *)(buf + o_pa);
+    cudaEvent_t ev[3] = {};
+    for (auto &e : ev) ICNV_CUDA(cudaEventCreate(&e));
+    auto body = [&]() -> int {
+        int rc2;
+        if ((rc2 = bm.upload(mp, st))) return rc2;
+        ICNV_CUDA(cudaEventRecord(ev[0], st));
+        if ((rc2 = bm.bh(p_raw, G, npair, p_thresh, PA, st))) return rc2;
+        ICNV_CUDA(cudaEventRecord(ev[1], st));
+        if ((rc2 = bm.mask(X, ldx, Y, ldy, G, C, n_ref, rule, mask_val, st))) return rc2;
+        ICNV_CUDA(cudaEventRecord(ev[2], st));
+        ICNV_CUDA(cudaStreamSynchronize(st));
+        float ms = 0.0f;
+        for (int s = 0; s < 2 && times; ++s) {
+            ICNV_CUDA(cudaEventElapsedTime(&ms, ev[s], ev[s + 1]));
+            times[s] += ms;
+        }
+        return ICNV_OK;
+    };
+    rc = body();
+    cudaFreeAsync(buf, st);
+    for (auto &e : ev)
+        if (e) cudaEventDestroy(e);
+    return rc;
 }
 
 }  // namespace icnv

@@ -16,6 +16,8 @@ import torch
 from . import _lib, dist as shard
 from .api import _i32, groups_to_csr
 
+_E_NONFINITE = -5   # ICNV_E_NONFINITE
+
 
 def _stream_ptr():
     """torch's current stream as the `void *stream` of the device ABI.  torch's default stream is
@@ -485,6 +487,130 @@ class Engine:
             float(p_val_thresh), _code(DE_RULES, rule, "rule"), float(center_val), float(jitter_mean), float(jitter_sd),
             int(seed) & 0xFFFFFFFFFFFFFFFF, p_raw.data_ptr() if npair else None, p_adj.data_ptr() if npair else None,
             _stream_ptr()))
+        return Y, p_raw, p_adj
+
+    def _all_to_all(self, out: torch.Tensor, inp: torch.Tensor, out_splits, in_splits) -> None:
+        """all_to_all_single of flat tensors.  NCCL: on torch's current stream; any other backend through host memory, as
+        _all_gather - same bytes, same order."""
+        import torch.distributed as tdist
+        if tdist.get_backend() == "nccl":
+            tdist.all_to_all_single(out, inp, out_splits, in_splits)
+            return
+        host = torch.empty(out.shape, dtype=out.dtype)
+        tdist.all_to_all_single(host, inp.detach().cpu(), out_splits, in_splits)
+        out.copy_(host.to(out.device))
+
+    def mask_non_de_sharded(self, X_local, ref_groups_local, subclusters_local, test="wilcoxon", p_val_thresh=0.05, rule="any",
+                            center_val=None, jitter_mean=1e-4, jitter_sd=1e-4, seed=0, out=None, slab_genes=None):
+        """mask_non_DE_genes_basic on a cell shard: X_local is this rank's resident (C_local, G) float64 tensor with contiguous
+        genes; ref_groups_local / subclusters_local are, per group, this rank's LOCAL columns (the planner's slices, possibly
+        empty), so rank order restores each group's global list order (as mean_sd).  Each rank owns a contiguous range of
+        genes: the listed cells are packed for every rank's range and exchanged (all-to-all) in gene sub-slabs sized from free
+        memory (`slab_genes` forces the size), each rank tests its genes, the p rows are all-gathered, and every rank runs BH
+        on all of them and masks its own cells.  Returns (Y_local, p_raw, p_adj): p_raw / p_adj the whole (n_pairs, G) on
+        every rank, row s * n_ref + j.  The bytes equal api.mask_non_de_genes on the gathered matrix with the same seed and
+        center_val, for any number of ranks.  center_val defaults to the mean over all ranks, combined in a fixed order
+        (icnv_combine_cell_stats), so it does not depend on the number of ranks either.  NaN / Inf in a listed cell of any
+        rank raises ICNV_E_NONFINITE on every rank."""
+        import torch.distributed as tdist
+        from .api import DE_RULES, DE_TESTS, _code
+        if X_local.dtype != torch.float64 or X_local.dim() != 2 or (X_local.shape[1] > 1 and X_local.stride(1) != 1):
+            raise ValueError("X_local must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X_local.shape
+        world = self._world()
+        rank = tdist.get_rank() if world > 1 else 0
+        refs = [np.asarray(g, dtype=np.int32) for g in ref_groups_local]
+        subs = [np.asarray(g, dtype=np.int32) for g in subclusters_local]
+        n_ref, n_sub = len(refs), len(subs)
+        npair, ng = n_ref * n_sub, n_ref + n_sub
+        test_c, rule_c = _code(DE_TESTS, test, "test"), _code(DE_RULES, rule, "rule")
+        mine = np.concatenate(refs + subs) if ng and sum(len(g) for g in refs + subs) else np.zeros(0, np.int32)
+        if mine.size and (mine.min() < 0 or mine.max() >= C):
+            raise ValueError("a listed column is outside this rank's cells")
+        if center_val is None:
+            center_val = self.mean_sd(X_local.contiguous(), [np.arange(C, dtype=np.int32)])[0]
+        # every rank's entry count per group -> global group offsets and each rank's list positions
+        lens = np.asarray([len(g) for g in refs + subs], dtype=np.int64)
+        if world > 1:
+            all_lens = np.stack([t.cpu().numpy() for t in self._all_gather_list(torch.as_tensor(lens, device=self.tdev))])
+        else:
+            all_lens = lens[None, :]
+        sizes = all_lens.sum(axis=0)
+        if n_ref < 1 or (sizes == 0).any():
+            raise ValueError("every reference group and subcluster needs at least one cell on some rank")
+        goff = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        T = int(goff[-1])
+        m = all_lens.sum(axis=1)                                         # listed entries per rank
+        gb = [G * d // world for d in range(world + 1)]                  # rank d tests genes [gb[d], gb[d + 1])
+        n_max = max(gb[d + 1] - gb[d] for d in range(world))
+        Y = torch.empty_like(X_local) if out is None else out
+        p_raw = torch.empty((npair, G), dtype=torch.float64, device=self.tdev)
+        p_adj = torch.empty((npair, G), dtype=torch.float64, device=self.tdev)
+        if npair:
+            roff = goff[:n_ref + 1].astype(np.int32)
+            soff = (goff[n_ref:] - goff[n_ref]).astype(np.int32)
+            # received entries in source order, each tagged with its global list position
+            tags = np.concatenate([goff[k] + all_lens[:q, k].sum() + np.arange(all_lens[q, k]) for q in range(world)
+                                   for k in range(ng)]).astype(np.int32)
+            d_tags = torch.as_tensor(tags, device=self.tdev)
+            d_cols = torch.as_tensor(mine if mine.size else np.zeros(1, np.int32), device=self.tdev)
+            src_m = np.ascontiguousarray(m, dtype=np.int64)
+            flag = torch.zeros(1, dtype=torch.int32, device=self.tdev)
+            if slab_genes is None:
+                # per gene of a sub-slab: send (at most world blocks of this rank's entries), receive, slab rows, the tests'
+                # scratch (a sorted reference row, group statistics) and the p slab
+                per_gene = 8 * (world * int(m[rank]) + 2 * T + int(goff[n_ref]) + 3 * ng + npair)
+                free, _ = torch.cuda.mem_get_info(self.tdev)
+                slab = max(1, min(n_max, (free - (1 << 30)) // per_gene))
+                if world > 1:
+                    slab = int(min(int(t.item()) for t in self._all_gather_list(torch.tensor([slab], device=self.tdev))))
+            else:
+                slab = max(1, int(slab_genes))
+            p_loc = torch.empty((npair, max(n_max, 1)), dtype=torch.float64, device=self.tdev)
+            for s0 in range(0, n_max, slab):
+                lo = np.asarray([min(gb[d] + s0, gb[d + 1]) for d in range(world)], dtype=np.int64)
+                hi = np.asarray([min(gb[d] + s0 + slab, gb[d + 1]) for d in range(world)], dtype=np.int64)
+                n_s = int(hi[rank] - lo[rank])
+                send = torch.empty(int((hi - lo).sum()) * int(m[rank]), dtype=torch.float64, device=self.tdev)
+                _lib.check(self.lib.icnv_dev_de_pack_f64(X_local.data_ptr(), max(X_local.stride(0), G), d_cols.data_ptr(),
+                                                         int(m[rank]), world, lo.ctypes.data, hi.ctypes.data,
+                                                         send.data_ptr(), flag.data_ptr(), _stream_ptr()))
+                if world > 1:
+                    recv = torch.empty(n_s * T, dtype=torch.float64, device=self.tdev)
+                    self._all_to_all(recv, send, [n_s * int(m[q]) for q in range(world)],
+                                     [int(hi[d] - lo[d]) * int(m[rank]) for d in range(world)])
+                else:
+                    recv = send
+                Z = torch.empty(n_s * T, dtype=torch.float64, device=self.tdev)
+                _lib.check(self.lib.icnv_dev_de_place_f64(recv.data_ptr(), n_s, world, src_m.ctypes.data, d_tags.data_ptr(), T,
+                                                          Z.data_ptr(), _stream_ptr()))
+                _lib.check(self.lib.icnv_dev_de_slab_tests_f64(
+                    Z.data_ptr(), T, int(lo[rank]), n_s, roff.ctypes.data, n_ref, soff.ctypes.data, n_sub, test_c,
+                    float(jitter_mean), float(jitter_sd), int(seed) & 0xFFFFFFFFFFFFFFFF, p_loc.data_ptr() + 8 * s0,
+                    p_loc.stride(0), _stream_ptr()))
+                del send, recv, Z
+            if world > 1:
+                self._all_reduce_sum(flag)
+            if int(flag.item()):
+                raise _lib.InfercnvB200Error(_E_NONFINITE, "mask_non_de_sharded: NaN or Inf in a listed cell")
+            if world > 1:
+                gathered = torch.empty((world,) + tuple(p_loc.shape), dtype=torch.float64, device=self.tdev)
+                self._all_gather(gathered, p_loc)
+                for d in range(world):
+                    p_raw[:, gb[d]:gb[d + 1]] = gathered[d, :, :gb[d + 1] - gb[d]]
+                del gathered
+            else:
+                p_raw.copy_(p_loc[:, :G])
+            del p_loc
+        # BH of every pair on every rank (deterministic), then the mask of this rank's cells
+        sub_size = np.ascontiguousarray(goff[n_ref + 1:] - goff[n_ref:-1], dtype=np.int32) if n_sub else np.zeros(1, np.int32)
+        ridx = np.concatenate(refs) if sum(len(g) for g in refs) else np.zeros(1, np.int32)
+        soff_l, sidx_l = groups_to_csr(subs)
+        _lib.check(self.lib.icnv_dev_de_bh_mask_f64(
+            p_raw.data_ptr() if npair else None, G, n_ref, n_sub, sub_size.ctypes.data, float(p_val_thresh),
+            p_adj.data_ptr() if npair else None, X_local.data_ptr() if C else None, max(X_local.stride(0), G),
+            Y.data_ptr() if C else None, max(Y.stride(0), G), C, _i32(ridx).ctypes.data, sum(len(g) for g in refs),
+            soff_l.ctypes.data, sidx_l.ctypes.data, rule_c, float(center_val), _stream_ptr()))
         return Y, p_raw, p_adj
 
     def bayesnet(self, X, regions_genes, regions_cells, mu, tau, n_chains, n_burn=700, n_keep=1000, seed=0, pooled=None,
