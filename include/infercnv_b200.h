@@ -309,6 +309,35 @@ ICNV_API int icnv_random_tree_heights_f64(const double *X, int64_t G, int64_t C,
  * linkages} (device time summed over the waves); zeros before any call. */
 ICNV_API int icnv_debug_random_trees(double *out5);
 
+/* The z-score gene filter of define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:45-68) on the G x C matrix X:
+ *   ref = X[, ref_idx] (n_ref 0-based columns, unlist(reference_grouped_cell_indices) in that order),
+ *   z = (ref - mean(ref)) / sd(ref),   outlier[g] = 1 when mean(|z[g, ]|) >= 0.8, else 0.
+ * mean(ref) / sd(ref) are icnv_mean_sd_f64's bits for the same list; each z is |__ddiv_rn(x - mu, sigma)|, and the row mean
+ * is the correctly rounded mean of those values (R's long-double mean() with its refinement pass, restated with
+ * double-double sums).  The threshold is the literal 0.8; a constant reference (sigma = 0, every z NaN) flags no gene.
+ * G < 2, n_ref < 1 or an index outside [0, C): ICNV_E_BAD_ARG; NaN / Inf in a listed column: ICNV_E_NONFINITE. */
+ICNV_API int icnv_zscore_outlier_genes_f64(const double *X, int64_t G, int64_t C, const int32_t *ref_idx, int64_t n_ref,
+                                           uint8_t *outlier);
+
+/* Every tree of define_signif_tumor_subclusters in one call: for each group k (CSR: 0-based columns
+ * grp_idx[grp_off[k] .. grp_off[k+1]) of the G x C matrix X) with n_k >= 2 cells,
+ *   hclust(parallelDist(t(X[keep, cells_k])), method) - icnv_pairwise_dist_f64 -> icnv_hclust_f64 on that group, bit for bit.
+ * keep: n_keep 0-based genes (any order); NULL means all G genes, and an empty list (n_keep = 0, keep != NULL) means none,
+ * so every distance is 0 (expr.data[-integer(0), ] keeps no row).  Outputs are packed in group order: the trees of the groups
+ * before k take R_k = sum of (n_j - 1) over those of them with n_j >= 2 rows, and group k's merge ((n_k - 1) x 2,
+ * column-major) is at merge + 2 R_k, its height at height + R_k, its order (1-based) at order + grp_off[k].  A group of one
+ * cell gets order 1 and no row; an empty group gets nothing.  Only the listed columns go to the device.  The groups run as
+ * the linkages of waves of at most one group per SM (largest first, as many as fit the free device memory); the result does
+ * not depend on the waves.  Methods as icnv_hclust_f64.  Centroid / median or a group of more than 65536 cells:
+ * ICNV_E_UNSUPPORTED, before anything is allocated; another method code, an index out of range or descending offsets:
+ * ICNV_E_BAD_ARG; NaN / Inf in a used column (or an infinite distance): ICNV_E_NONFINITE. */
+ICNV_API int icnv_cluster_groups_f64(const double *X, int64_t G, int64_t C, const int32_t *keep, int64_t n_keep,
+                                     const int32_t *grp_off, const int32_t *grp_idx, int n_grp, int method, int32_t *merge,
+                                     double *height, int32_t *order);
+/* What the last group-trees call did: out5 = {waves, groups in the largest wave, ms of the gene gather, ms of distances,
+ * ms of linkages} (device time summed over the waves); zeros before any call and after a call without a tree. */
+ICNV_API int icnv_debug_cluster_groups(double *out5);
+
 /* mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52; run() step 21, R/inferCNV_ops.R:1509-1524) on the G x C matrix X:
  * get_DE_genes_basic's tests, BH and .mask_DE_genes' mask in one call.
  *   Groups (CSR, 0-based columns): n_ref >= 1 reference groups; n_sub >= 0 TESTED subclusters in R's loop order (observation
@@ -583,6 +612,17 @@ ICNV_API int icnv_dev_hclust_f64(const double *d_dist, int64_t n, int method, in
 ICNV_API int icnv_dev_random_tree_heights_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
                                               int window, int method, int n_perm, uint64_t seed, int32_t *merge,
                                               double *height, double *perm_max_height, void *stream);
+/* icnv_zscore_outlier_genes_f64 on device pointers: X is G x (columns) with ld G, d_ref_idx n_ref device indices, outlier
+ * G bytes (device).  Synchronises `stream` twice: the per-cell statistics are combined on the host, then the non-finite check. */
+ICNV_API int icnv_dev_zscore_outlier_genes_f64(const double *X, int64_t G, const int32_t *d_ref_idx, int64_t n_ref,
+                                               uint8_t *outlier, void *stream);
+/* icnv_cluster_groups_f64 on device pointers: X (column stride ldx >= G, C columns), d_keep (device; NULL: all genes),
+ * grp_off (HOST), d_grp_idx (device), merge / height (device, packed as above), no order (icnv_hclust_order on the host
+ * copy of each group's merge).  With a keep list the kept rows of all C columns are gathered once (n_keep x C doubles).
+ * Synchronises `stream` once to check the indices, once per wave after its distances (non-finite check) and at the end. */
+ICNV_API int icnv_dev_cluster_groups_f64(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep,
+                                         int64_t n_keep, const int32_t *grp_off /*host*/, const int32_t *d_grp_idx, int n_grp,
+                                         int method, int32_t *merge, double *height, void *stream);
 /* icnv_mask_non_de_f64 on device pointers: X (column stride ldx >= G), Y (ldy >= G; may be X, nullable), p_raw / p_adj
  * (G x (n_sub n_ref), nullable); the group lists are HOST arrays.  Synchronises `stream` after each gene tile (non-finite
  * check) and at the end. */

@@ -452,6 +452,59 @@ def random_trees_stats() -> dict:
     return {"B": int(out[0]), "waves": int(out[1]), "prep_ms": out[2], "dist_ms": out[3], "link_ms": out[4]}
 
 
+def zscore_outlier_genes(X, ref_cells) -> np.ndarray:
+    """The z-score gene filter of define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:45-68) on the genes x cells
+    matrix X: a boolean mask of the genes with mean(|z|) >= 0.8 over the reference columns `ref_cells` (in that order), z
+    standardised by api.mean_sd's mu and sigma of those columns (icnv_zscore_outlier_genes_f64)."""
+    X = _f64(X)
+    G, C = X.shape
+    idx = _i32(ref_cells)
+    out = np.empty(G, dtype=np.uint8)
+    _lib.check(_lib.load().icnv_zscore_outlier_genes_f64(_p(X), G, C, _p(idx), len(idx), _p(out)))
+    return out.astype(bool)
+
+
+def _tree_split(merge, height, order, sizes):
+    """The packed outputs of icnv_cluster_groups_f64 -> one (merge, height, order) per group."""
+    trees, r, o = [], 0, 0
+    for n in sizes:
+        nm = max(n - 1, 0)
+        m = np.asfortranarray(merge[2 * r:2 * r + 2 * nm].reshape((nm, 2), order="F"))
+        trees.append((m, height[r:r + nm].copy(), order[o:o + n].copy()))
+        r += nm
+        o += n
+    return trees
+
+
+def cluster_groups(X, groups, method="ward.D2", keep=None):
+    """hclust(parallelDist(t(X[keep, g])), method) for every cell list g of `groups` (columns of the genes x cells matrix X)
+    in one call (icnv_cluster_groups_f64): a list of (merge, height, order), each bit-identical to
+    hclust(pairwise_dist(X[keep], g), method).  keep: genes to use (default all; an empty list uses none, so every distance
+    is 0).  A group of fewer than 2 cells gets an empty merge / height and order 1 .. n."""
+    X = _f64(X)
+    G, C = X.shape
+    off, idx = groups_to_csr(groups)
+    sizes = np.diff(off).tolist()
+    k = None if keep is None else _i32(keep)
+    kp = np.zeros(1, np.int32) if k is not None and k.size == 0 else k   # non-NULL: "no genes", never read
+    rows = sum(max(n - 1, 0) for n in sizes)
+    merge = np.empty(max(2 * rows, 1), dtype=np.int32)
+    height = np.empty(max(rows, 1), dtype=np.float64)
+    order = np.empty(max(int(off[-1]), 1), dtype=np.int32)
+    _lib.check(_lib.load().icnv_cluster_groups_f64(
+        _p(X), G, C, _p(kp), 0 if k is None else len(k), _p(off), _p(idx), len(sizes), hclust_method_code(method), _p(merge), _p(height),
+        _p(order)))
+    return _tree_split(merge, height, order, sizes)
+
+
+def cluster_groups_stats() -> dict:
+    """What the last cluster_groups call did: waves, groups in the largest wave, device ms of the gene gather, the distances
+    and the linkages (icnv_debug_cluster_groups)."""
+    out = np.zeros(5, dtype=np.float64)
+    _lib.check(_lib.load().icnv_debug_cluster_groups(_p(out)))
+    return {"waves": int(out[0]), "widest": int(out[1]), "gather_ms": out[2], "dist_ms": out[3], "link_ms": out[4]}
+
+
 DE_TESTS = {"wilcoxon": 0, "t": 1}
 DE_RULES = {"any": 0, "most": 1, "all": 2}
 

@@ -580,6 +580,27 @@ static int upload_matrix(const double *X, int64_t n, double **dX, int slot, cuda
     return ICNV_OK;
 }
 
+// The columns idx[0 .. n) of the host matrix X (G rows) into a compact device buffer (SLOT_IN), each run of consecutive
+// indices as one copy, and the identity list 0 .. n-1 into SLOT_IDX.  The caller has checked the indices.
+static int upload_listed_columns(const double *X, int64_t G, const int32_t *idx, int64_t n, double **dX, int32_t **d_ident,
+                                 cudaStream_t st) {
+    *dX = (double *)scratch(SLOT_IN, sizeof(double) * (size_t)std::max<int64_t>(G * n, 1));
+    *d_ident = (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * (size_t)n);
+    if (!*dX || !*d_ident) return ICNV_E_NOMEM;
+    std::vector<int32_t> ident((size_t)n);
+    std::iota(ident.begin(), ident.end(), 0);
+    for (int64_t i = 0; G > 0 && i < n;) {
+        int64_t j = i + 1;
+        while (j < n && idx[j] == idx[j - 1] + 1) ++j;
+        ICNV_CUDA(cudaMemcpyAsync(*dX + G * i, X + G * (int64_t)idx[i], sizeof(double) * (size_t)G * (size_t)(j - i),
+                                  cudaMemcpyHostToDevice, st));
+        i = j;
+    }
+    ICNV_CUDA(cudaMemcpyAsync(*d_ident, ident.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));   // `ident` is pageable host memory that goes out of scope
+    return ICNV_OK;
+}
+
 int icnv_ref_means_f64(const double *X, int64_t G, int64_t C, const int32_t *grp_off, const int32_t *grp_idx, int n_grp,
                        int inv_log, double *means) {
     ICNV_HOST_PROLOGUE();
@@ -1708,23 +1729,14 @@ int icnv_mean_sd_f64(const double *X, int64_t G, int64_t C, const int32_t *idx, 
         return set_error(ICNV_E_BAD_ARG, "icnv_mean_sd_f64: bad argument");
     for (int64_t i = 0; i < n_idx; ++i)
         if (idx[i] < 0 || idx[i] >= C) return set_error(ICNV_E_BAD_ARG, "cell index out of range");
-    // only the listed columns go to the device (the reference cells are a tenth of the matrix): runs of consecutive
-    // indices as one copy each into a compact buffer, the statistics then run over its columns 0 .. n_idx-1
+    // only the listed columns go to the device (the reference cells are a tenth of the matrix); the statistics then run over
+    // the compact buffer's columns 0 .. n_idx-1
     int rc;
-    double *dX = (double *)scratch(SLOT_IN, sizeof(double) * (size_t)G * (size_t)n_idx);
-    int32_t *d_idx = (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * (size_t)n_idx);
+    double *dX = nullptr;
+    int32_t *d_idx = nullptr;
     double *d_stats = (double *)scratch(SLOT_MEANS, sizeof(double) * 2 * (size_t)n_idx);
-    if (!dX || !d_idx || !d_stats) return ICNV_E_NOMEM;
-    std::vector<int32_t> ident((size_t)n_idx);
-    for (int64_t i = 0; i < n_idx;) {
-        int64_t j = i + 1;
-        while (j < n_idx && idx[j] == idx[j - 1] + 1) ++j;
-        ICNV_CUDA(cudaMemcpyAsync(dX + G * i, X + G * (int64_t)idx[i], sizeof(double) * (size_t)G * (size_t)(j - i), cudaMemcpyHostToDevice, st));
-        for (int64_t k = i; k < j; ++k) ident[(size_t)k] = (int32_t)k;
-        i = j;
-    }
-    idx = ident.data();
-    ICNV_CUDA(cudaMemcpyAsync(d_idx, idx, sizeof(int32_t) * (size_t)n_idx, cudaMemcpyHostToDevice, st));
+    if (!d_stats) return ICNV_E_NOMEM;
+    if ((rc = upload_listed_columns(X, G, idx, n_idx, &dX, &d_idx, st))) return rc;
     // per-cell sum and sd on the device; the n_idx-vectors are combined in list order (the same
     // combination the multi-GPU driver applies to all-gathered per-cell statistics: identical bits)
     if ((rc = icnv_dev_column_stats_f64(dX, G, d_idx, n_idx, d_stats, d_stats + n_idx, st))) return rc;
@@ -2235,6 +2247,112 @@ int icnv_dev_smooth_coordinates_f64(const double *X, int64_t ldx, double *Y, int
     if (rc) return rc;
     return icnv::smooth_coords_dev(X, ldx, Y, ldy, G, C, chr_start, chr_len, K, gene_start, gene_stop, window_length,
                                    pick_stream(stream), who);
+}
+
+}  // extern "C"
+
+// ---- subclustering trees, K17 (kernels and device bodies in icnv_subclusters.cu) -------------------------------------------
+// Weak references, as for the linkage: a build without icnv_subclusters.cu reports them as unsupported.
+namespace icnv {
+int zscore_outlier_dev(const double *X, int64_t G, const int32_t *d_cells, int64_t n, uint8_t *outlier, void *stream,
+                       const char *who) __attribute__((weak));
+int cluster_groups_check(int64_t G, const int32_t *keep, int64_t n_keep, const int32_t *grp_off, int n_grp, int method,
+                         const char *who) __attribute__((weak));
+int64_t cluster_groups_rows(const int32_t *grp_off, int n_grp) __attribute__((weak));
+int cluster_groups_dev(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep, int64_t n_keep,
+                       const int32_t *grp_off, const int32_t *d_idx, int n_grp, int method, int32_t *merge, double *height,
+                       void *stream, const char *who) __attribute__((weak));
+void cluster_groups_stats(double *out5) __attribute__((weak));
+
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_zscore_outlier_genes_f64(const double *X, int64_t G, int64_t C, const int32_t *ref_idx, int64_t n_ref,
+                                  uint8_t *outlier) {
+    static const char *who = "icnv_zscore_outlier_genes_f64";
+    if (!icnv::zscore_outlier_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no z-score filter kernel", who);
+    ICNV_HOST_PROLOGUE();
+    if (!X || !ref_idx || !outlier || G <= 1 || C <= 0 || n_ref <= 0) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    for (int64_t i = 0; i < n_ref; ++i)
+        if (ref_idx[i] < 0 || ref_idx[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index out of range", who);
+    double *dX = nullptr;
+    int32_t *d_idx = nullptr;
+    uint8_t *d_out = (uint8_t *)scratch(SLOT_OUT, (size_t)G);
+    if (!d_out) return ICNV_E_NOMEM;
+    int rc = upload_listed_columns(X, G, ref_idx, n_ref, &dX, &d_idx, st);
+    if (rc) return rc;
+    if ((rc = icnv::zscore_outlier_dev(dX, G, d_idx, n_ref, d_out, st, who))) return rc;
+    ICNV_CUDA(cudaMemcpyAsync(outlier, d_out, (size_t)G, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return ICNV_OK;
+}
+
+int icnv_dev_zscore_outlier_genes_f64(const double *X, int64_t G, const int32_t *d_ref_idx, int64_t n_ref, uint8_t *outlier,
+                                      void *stream) {
+    static const char *who = "icnv_dev_zscore_outlier_genes_f64";
+    if (!icnv::zscore_outlier_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no z-score filter kernel", who);
+    return icnv::zscore_outlier_dev(X, G, d_ref_idx, n_ref, outlier, stream, who);
+}
+
+int icnv_cluster_groups_f64(const double *X, int64_t G, int64_t C, const int32_t *keep, int64_t n_keep, const int32_t *grp_off,
+                            const int32_t *grp_idx, int n_grp, int method, int32_t *merge, double *height, int32_t *order) {
+    static const char *who = "icnv_cluster_groups_f64";
+    if (!icnv::cluster_groups_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no group-tree kernels", who);
+    int rc = icnv::cluster_groups_check(G, keep, n_keep, grp_off, n_grp, method, who);
+    if (rc) return rc;
+    ICNV_HOST_PROLOGUE();
+    const int64_t n_list = n_grp > 0 ? grp_off[n_grp] : 0, rows = icnv::cluster_groups_rows(grp_off, n_grp);
+    if (!X || C <= 0 || (n_list > 0 && (!grp_idx || !order)) || (rows > 0 && (!merge || !height)))
+        return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    for (int64_t i = 0; i < n_list; ++i)
+        if (grp_idx[i] < 0 || grp_idx[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index out of range", who);
+    for (int64_t i = 0; keep && i < n_keep; ++i)
+        if (keep[i] < 0 || keep[i] >= G) return set_error(ICNV_E_BAD_ARG, "%s: gene index out of range", who);
+    for (int k = 0; k < n_grp; ++k)
+        if (grp_off[k + 1] - grp_off[k] == 1) order[grp_off[k]] = 1;
+    if (rows == 0) return ICNV_OK;
+    double *dX = nullptr;
+    int32_t *d_idx = nullptr, *d_keep = nullptr;
+    double *d_height = (double *)scratch(SLOT_OUT, (sizeof(double) + 2 * sizeof(int32_t)) * (size_t)rows);
+    if (!d_height) return ICNV_E_NOMEM;
+    int32_t *d_merge = (int32_t *)(d_height + rows);
+    if ((rc = upload_listed_columns(X, G, grp_idx, n_list, &dX, &d_idx, st))) return rc;
+    if (keep) {   // an empty list still means "no genes": any non-NULL device pointer stands for it
+        d_keep = n_keep > 0 ? (int32_t *)scratch(SLOT_IDX2, sizeof(int32_t) * (size_t)n_keep) : d_idx;
+        if (!d_keep) return ICNV_E_NOMEM;
+        if (n_keep > 0) ICNV_CUDA(cudaMemcpyAsync(d_keep, keep, sizeof(int32_t) * (size_t)n_keep, cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = icnv::cluster_groups_dev(dX, G, G, n_list, d_keep, n_keep, grp_off, d_idx, n_grp, method, d_merge, d_height, st,
+                                       who)))
+        return rc;
+    ICNV_CUDA(cudaMemcpyAsync(merge, d_merge, sizeof(int32_t) * 2 * (size_t)rows, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaMemcpyAsync(height, d_height, sizeof(double) * (size_t)rows, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    int64_t r = 0;
+    for (int k = 0; k < n_grp; ++k) {
+        const int64_t n = (int64_t)grp_off[k + 1] - grp_off[k];
+        if (n < 2) continue;
+        if ((rc = icnv_hclust_order(merge + 2 * r, n, order + grp_off[k]))) return rc;
+        r += n - 1;
+    }
+    return ICNV_OK;
+}
+
+int icnv_dev_cluster_groups_f64(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep, int64_t n_keep,
+                                const int32_t *grp_off, const int32_t *d_grp_idx, int n_grp, int method, int32_t *merge,
+                                double *height, void *stream) {
+    static const char *who = "icnv_dev_cluster_groups_f64";
+    if (!icnv::cluster_groups_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no group-tree kernels", who);
+    return icnv::cluster_groups_dev(X, G, ldx, C, d_keep, n_keep, grp_off, d_grp_idx, n_grp, method, merge, height, stream,
+                                    who);
+}
+
+int icnv_debug_cluster_groups(double *out5) {
+    if (!out5) return set_error(ICNV_E_BAD_ARG, "icnv_debug_cluster_groups: out5 is NULL");
+    for (int i = 0; i < 5; ++i) out5[i] = 0.0;
+    if (icnv::cluster_groups_stats) icnv::cluster_groups_stats(out5);
+    return ICNV_OK;
 }
 
 }  // extern "C"

@@ -108,6 +108,15 @@ inline cudaError_t upload_if_changed(std::vector<unsigned char> &cache, cudaStre
     return cudaMemcpyAsync(dst, cache.data(), bytes, cudaMemcpyHostToDevice, st);
 }
 
+// One linkage of a member-table launch (K17: trees of groups of different sizes side by side).  Its cells are the list
+// entries cell_off .. cell_off + n - 1, its n x ld distance matrix starts at M + m_off (ld = n rounded up to even), its
+// linkage scratch at w8 + s8_off (n + P doubles) and w4 + s4_off (6 n + P int32; P = the power of two >= n - 1), and its
+// merge / height at merge + 2 out_off / height + out_off.  dist_square_kernel and hclust_nn_chain_kernel both read it.
+struct HcMember {
+    int64_t cell_off, n, ld, m_off, s8_off, s4_off, out_off;
+    int32_t P, pad;
+};
+
 Ctx &ctx();
 int set_error(int code, const char *fmt, ...);
 // grow-only device scratch; returns nullptr (and sets the error) on failure

@@ -158,27 +158,48 @@ __global__ void __launch_bounds__(PD_NT, 1) pairwise_dist_kernel(const DistParam
 // Member z = blockIdx.x / T (tile column blockIdx.x % T, T tiles per side): columns X + z * sx (ldx, no cell list), matrix M + z * sm (n x ld).  Entry (a, b), a != b, is the
 // value hclust_fill_kernel would store from pairwise_dist_kernel's entry of the pair, v = sqrt(sum) (v * v for ward.D2), in
 // both triangles; the diagonal is +inf.  flag |= 1 when a value is not finite, as that kernel reports it.
+// K17's members of different n (tiles != nullptr): a 1-D grid over a tile-work table, tiles[blockIdx.x] = (member, bi, bj)
+// with bi <= bj; the member's cells are d.cells + cell_off (X and ldx shared), its matrix M + m_off with its own ld.
 struct DistSqParams {
-    DistParams d;         // X, G, ldx, n, rows = 0, cells = out = nullptr
+    DistParams d;         // X, G, ldx, n, rows = 0, cells = out = nullptr (a member table: cells = the groups' lists)
     int64_t sx, sm, ld;
     unsigned T;
     double *M;
     int square;
     int *flag;
+    const int4 *tiles;
+    const HcMember *mem;
 };
 
 __global__ void __launch_bounds__(PD_NT, 1) dist_square_kernel(const DistSqParams q) {
-    const unsigned z = blockIdx.x / q.T;
-    const int bi = blockIdx.y, bj = (int)(blockIdx.x - z * q.T);
-    if (bi > bj) return;
+    int bi, bj;
+    int64_t n, ld;
+    DistParams p = q.d;
+    double *M;
+    if (q.tiles) {
+        const int4 t = q.tiles[blockIdx.x];
+        const HcMember m = q.mem[t.x];
+        bi = t.y;
+        bj = t.z;
+        n = p.n = m.n;
+        ld = m.ld;
+        p.cells += m.cell_off;
+        M = q.M + m.m_off;
+    } else {
+        const unsigned z = blockIdx.x / q.T;
+        bi = blockIdx.y;
+        bj = (int)(blockIdx.x - z * q.T);
+        if (bi > bj) return;
+        n = q.d.n;
+        ld = q.ld;
+        p.X += (int64_t)z * q.sx;
+        M = q.M + (int64_t)z * q.sm;
+    }
     extern __shared__ __align__(16) double pd_smem[];
     double *As = pd_smem;
     double *Bs = pd_smem + 2 * PD_T * PD_LD;
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int64_t i0 = (int64_t)bi * PD_T, j0 = (int64_t)bj * PD_T, n = q.d.n, ld = q.ld;
-    DistParams p = q.d;
-    p.X += (int64_t)z * q.sx;
-    double *M = q.M + (int64_t)z * q.sm;
+    const int64_t i0 = (int64_t)bi * PD_T, j0 = (int64_t)bj * PD_T;
     double acc[8][8];
     dist_tile(p, i0, j0, As, Bs, acc);
     bool bad = false;
@@ -206,10 +227,24 @@ int dist_square_launch(const double *X, int64_t G, int64_t ldx, int64_t sx, int6
                        int64_t sm, int square, int *flag, cudaStream_t st) {
     const int64_t T = (n + PD_T - 1) / PD_T;
     if (T > 65535) return set_error(ICNV_E_UNSUPPORTED, "distances: %lld cells (limit %d)", (long long)n, 65535 * PD_T);
-    DistSqParams q{{X, G, ldx, nullptr, n, nullptr, 0}, sx, sm, ld, (unsigned)T, M, square, flag};
+    DistSqParams q{{X, G, ldx, nullptr, n, nullptr, 0}, sx, sm, ld, (unsigned)T, M, square, flag, nullptr, nullptr};
     const size_t smem = sizeof(double) * 4 * PD_T * PD_LD;
     ICNV_CUDA(cudaFuncSetAttribute(dist_square_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dist_square_kernel<<<dim3((unsigned)(T * B), (unsigned)T), PD_NT, smem, st>>>(q);
+    ICNV_CHECK_LAUNCH("dist_square_kernel");
+    return ICNV_OK;
+}
+
+// K17: the n_tiles tiles of d_tiles (device; (member, bi, bj), bi <= bj) over the members d_mem (device), whose cells are
+// columns X + ldx d_cells[cell_off + a] (genes x cells) -> each member's matrix in M.
+int dist_square_members_launch(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, const int4 *d_tiles,
+                               int64_t n_tiles, const HcMember *d_mem, double *M, int square, int *flag, cudaStream_t st) {
+    if (n_tiles <= 0) return ICNV_OK;
+    if (n_tiles > 0x7fffffff) return set_error(ICNV_E_UNSUPPORTED, "distances: %lld tiles in one launch", (long long)n_tiles);
+    DistSqParams q{{X, G, ldx, d_cells, 0, nullptr, 0}, 0, 0, 0, 1u, M, square, flag, d_tiles, d_mem};
+    const size_t smem = sizeof(double) * 4 * PD_T * PD_LD;
+    ICNV_CUDA(cudaFuncSetAttribute(dist_square_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dist_square_kernel<<<(unsigned)n_tiles, PD_NT, smem, st>>>(q);
     ICNV_CHECK_LAUNCH("dist_square_kernel");
     return ICNV_OK;
 }

@@ -89,6 +89,9 @@ struct HcParams {
     // a batched launch runs one linkage per CTA: member z = blockIdx.x works on M + z sM, raw_h / skey + z s8,
     // chain .. sidx + z s4, merge + z 2 (n - 1) and height + z (n - 1)
     int64_t sM, s8, s4;
+    // or, members of different n (K17): member z = blockIdx.x takes n, ld, P and its offsets from mem[z] (raw_h and chain
+    // are then the bases of the 8-byte and the int32 scratch)
+    const HcMember *mem;
 };
 
 __device__ __forceinline__ double lance_williams(int method, double dki, double dkj, double dij, double ni, double nj,
@@ -147,20 +150,38 @@ __global__ void __launch_bounds__(256) hclust_mirror_kernel(double *M, int64_t n
 
 __global__ void __launch_bounds__(HC_NT, 1) hclust_nn_chain_kernel(const HcParams p0) {
     HcParams p = p0;
-    {
-        const int64_t z = blockIdx.x;
-        p.M += z * p0.sM;
-        p.raw_h += z * p0.s8;
-        p.skey += z * p0.s8;
-        p.chain += z * p0.s4;
-        p.size += z * p0.s4;
-        p.raw_i += z * p0.s4;
-        p.raw_j += z * p0.s4;
-        p.uf += z * p0.s4;
-        p.node += z * p0.s4;
-        p.sidx += z * p0.s4;
-        p.merge += z * 2 * (p0.n - 1);
-        p.height += z * (p0.n - 1);
+    {   // both layouts keep a member's scratch as [raw_h | skey] (n + P doubles) and [chain | size | raw_i | raw_j | uf | node |
+        // sidx] (6 n + P int32) from its two bases
+        int64_t oM, o8, o4, oo;
+        if (p0.mem) {
+            const HcMember m = p0.mem[blockIdx.x];
+            p.n = m.n;
+            p.ld = m.ld;
+            p.P = m.P;
+            oM = m.m_off;
+            o8 = m.s8_off;
+            o4 = m.s4_off;
+            oo = m.out_off;
+        } else {
+            const int64_t z = blockIdx.x;
+            oM = z * p0.sM;
+            o8 = z * p0.s8;
+            o4 = z * p0.s4;
+            oo = z * (p0.n - 1);
+        }
+        const int64_t n = p.n;
+        p.M += oM;
+        p.raw_h += o8;
+        p.skey = reinterpret_cast<unsigned long long *>(p.raw_h + n);
+        p.chain += o4;
+        p.size = p.chain + n;
+        p.raw_i = p.chain + 2 * n;
+        p.raw_j = p.chain + 3 * n;
+        p.uf = p.chain + 4 * n;
+        p.node = p.chain + 5 * n;
+        p.sidx = p.chain + 6 * n;
+        p.merge += 2 * oo;
+        p.height += oo;
     }
     extern __shared__ __align__(16) unsigned char hc_smem[];
     double *buf = reinterpret_cast<double *>(hc_smem);                    // [HC_S][HC_CH]
@@ -384,32 +405,49 @@ int hclust_batch(double *M, int64_t n, int method, int B, int32_t *merge, double
     const size_t b8 = sizeof(double) * (size_t)s8 * (size_t)B, b4 = sizeof(int32_t) * (size_t)s4 * (size_t)B;
     char *w = nullptr;
     ICNV_CUDA(cudaMallocAsync((void **)&w, b8 + b4 + 64, st));
-    HcParams q;
+    HcParams q{};
     q.M = M;
     q.n = n;
     q.ld = ld;
     q.method = method;
-    q.raw_h = (double *)w;
-    q.skey = (unsigned long long *)(w + sizeof(double) * (size_t)n);
-    int32_t *i4 = (int32_t *)(w + b8);
-    q.chain = i4;
-    q.size = i4 + n;
-    q.raw_i = i4 + 2 * n;
-    q.raw_j = i4 + 3 * n;
-    q.uf = i4 + 4 * n;
-    q.node = i4 + 5 * n;
-    q.sidx = i4 + 6 * n;
+    q.raw_h = (double *)w;            // the kernel derives skey and size .. sidx from these two bases
+    q.chain = (int32_t *)(w + b8);
     q.merge = merge;
     q.height = height;
     q.P = P;
     q.sM = n * ld;
     q.s8 = s8;
     q.s4 = s4;
+    q.mem = nullptr;
     const size_t smem = sizeof(double) * HC_S * HC_CH + (size_t)((n + 15) & ~15);
     ICNV_CUDA(cudaFuncSetAttribute(hclust_nn_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     hclust_nn_chain_kernel<<<B, HC_NT, smem, st>>>(q);
     ICNV_CHECK_LAUNCH("hclust_nn_chain_kernel");
     ICNV_CUDA(cudaFreeAsync(w, st));
+    return ICNV_OK;
+}
+
+// K17: B linkages of members of different n in one launch, one CTA each (member z = d_mem[z], device).  The filled
+// matrices are at M + m_off, the scratch at w8 + s8_off / w4 + s4_off, the results at merge / height + the member's
+// out_off.  Dynamic shared memory is sized by n_max, the largest member's n.  Every member is the same function of its
+// own matrix as a single-tree launch.
+int hclust_member_batch(const HcMember *d_mem, int B, int64_t n_max, int method, double *M, double *w8, int32_t *w4,
+                        int32_t *merge, double *height, cudaStream_t st) {
+    if (B <= 0) return ICNV_OK;
+    HcParams q{};
+    q.M = M;
+    q.n = n_max;
+    q.ld = hclust_ld(n_max);
+    q.method = method;
+    q.raw_h = w8;
+    q.chain = w4;
+    q.merge = merge;
+    q.height = height;
+    q.mem = d_mem;
+    const size_t smem = sizeof(double) * HC_S * HC_CH + (size_t)((n_max + 15) & ~15);
+    ICNV_CUDA(cudaFuncSetAttribute(hclust_nn_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    hclust_nn_chain_kernel<<<B, HC_NT, smem, st>>>(q);
+    ICNV_CHECK_LAUNCH("hclust_nn_chain_kernel");
     return ICNV_OK;
 }
 

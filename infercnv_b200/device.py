@@ -448,6 +448,51 @@ class Engine:
         m = merge.cpu().numpy().T
         return m, height.cpu().numpy(), hclust_order(m), perm_max.cpu().numpy()
 
+    def zscore_outlier_genes(self, X, ref_cells):
+        """api.zscore_outlier_genes on the resident (C, G) float64 tensor X (rows = cells, contiguous): a boolean device
+        tensor of G genes, bit-identical to the host call."""
+        if X.dtype != torch.float64 or X.dim() != 2 or not X.is_contiguous():
+            raise ValueError("X must be a contiguous (cells, genes) float64 tensor")
+        G = X.shape[1]
+        idx = torch.as_tensor(np.asarray(ref_cells, dtype=np.int32), device=self.tdev)
+        out = torch.empty(G, dtype=torch.uint8, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_zscore_outlier_genes_f64(X.data_ptr(), G, idx.data_ptr(), int(idx.numel()), out.data_ptr(),
+                                                              _stream_ptr()))
+        return out.bool()
+
+    def cluster_groups(self, X, groups, method="ward.D2", keep=None):
+        """api.cluster_groups on the resident (C, G) float64 tensor X with contiguous genes: one (merge, height, order) per
+        group as numpy arrays, bit-identical to the host call.  keep: gene indices (host list or device tensor)."""
+        from .api import _tree_split, hclust_method_code, hclust_order
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X.shape
+        off, idx = groups_to_csr(groups)
+        sizes = np.diff(off).tolist()
+        d_idx = torch.as_tensor(idx, device=self.tdev)
+        d_keep = None
+        if keep is not None:
+            d_keep = torch.as_tensor(np.asarray(keep.cpu() if torch.is_tensor(keep) else keep, dtype=np.int32), device=self.tdev)
+        n_keep = 0 if d_keep is None else int(d_keep.numel())
+        if d_keep is not None and n_keep == 0:
+            d_keep = torch.zeros(1, dtype=torch.int32, device=self.tdev)   # non-NULL: "no genes", never read
+        rows = sum(max(n - 1, 0) for n in sizes)
+        merge = torch.empty(max(2 * rows, 1), dtype=torch.int32, device=self.tdev)
+        height = torch.empty(max(rows, 1), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_cluster_groups_f64(
+            X.data_ptr(), G, max(X.stride(0), G), C, None if d_keep is None else d_keep.data_ptr(), n_keep, off.ctypes.data,
+            d_idx.data_ptr(), len(sizes), hclust_method_code(method), merge.data_ptr(), height.data_ptr(), _stream_ptr()))
+        m, h = merge.cpu().numpy(), height.cpu().numpy()
+        order = np.empty(max(int(off[-1]), 1), dtype=np.int32)
+        r = 0
+        for k, n in enumerate(sizes):
+            if n >= 2:
+                order[off[k]:off[k] + n] = hclust_order(m[2 * r:2 * r + 2 * (n - 1)].reshape((n - 1, 2), order="F"))
+                r += n - 1
+            elif n == 1:
+                order[off[k]] = 1
+        return _tree_split(m, h, order, sizes)
+
     def smooth_coordinates(self, X, chr_start, chr_len, gene_start, gene_stop, window_length, out=None):
         """smooth_by_chromosome_coordinates on the resident (C, G) float64 tensor X with contiguous genes, as
         api.smooth_coordinates and bit-identical to it: returns Y (C, G), `out` or a new tensor (never X itself)."""

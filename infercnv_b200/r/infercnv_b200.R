@@ -776,6 +776,236 @@ b200_inferCNVBayesNet <- function( file_dir,
     obj
 }
 
+## define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:2-177), run() step 15, and its hidden-spike mirror: the
+## z-score gene filter (:45-68) and every hclust() tree of the step in GPU calls - one icnvR_zscore_outlier_genes, then one
+## icnvR_cluster_groups for all groups (and, with Leiden, all partitions), so no distance vector passes through R.  Same
+## signature and result as the original.  The filter keeps the original's quirk: which() never returns NULL, so with no outlier
+## gene expr.data[-outliers, ] keeps no gene and every distance is 0.
+##   qnorm / pheight / qgamma / none: cut heights and cutree() are R's own on the returned trees.
+##   leiden: the partition of every group is computed first, in group order, by the original's own
+##   .leiden_seurat_preprocess_routine / .leiden_simple_snn, so R's RNG is consumed as the original consumes it (the trees use
+##   none of it); then one call builds every partition's tree (and the whole group when k_nn >= its size), and the phylo
+##   assembly runs in the original's partition order.  The per-chromosome part stays the original's
+##   .whole_dataset_leiden_subclustering_per_chr on the filtered data (its nn2() is b200_nn2).
+## Falls back to the original for restrict_to_DE_genes = TRUE, a method outside the six, an unknown partition_method, a
+## non-double or NA-holding matrix, a group of more than 65 536 cells, or a library error.
+b200_define_signif_tumor_subclusters <- function(infercnv_obj, p_val = 0.1, k_nn = 20, leiden_method = c("PCA", "simple"),
+                                                 leiden_function = c("CPM", "modularity"), leiden_resolution = "auto",
+                                                 leiden_method_per_chr = c("simple", "PCA"),
+                                                 leiden_function_per_chr = c("modularity", "CPM"),
+                                                 leiden_resolution_per_chr = 1, hclust_method = "ward.D2",
+                                                 cluster_by_groups = TRUE, partition_method = "leiden",
+                                                 per_chr_hmm_subclusters = FALSE,
+                                                 per_chr_hmm_subclusters_references = FALSE, z_score_filter = 0.8,
+                                                 restrict_to_DE_genes = FALSE) {
+    orig <- .icnv_env$orig$define_signif_tumor_subclusters
+    call_orig <- function() orig(infercnv_obj, p_val = p_val, k_nn = k_nn, leiden_method = leiden_method,
+                                 leiden_function = leiden_function, leiden_resolution = leiden_resolution,
+                                 leiden_method_per_chr = leiden_method_per_chr, leiden_function_per_chr = leiden_function_per_chr,
+                                 leiden_resolution_per_chr = leiden_resolution_per_chr, hclust_method = hclust_method,
+                                 cluster_by_groups = cluster_by_groups, partition_method = partition_method,
+                                 per_chr_hmm_subclusters = per_chr_hmm_subclusters,
+                                 per_chr_hmm_subclusters_references = per_chr_hmm_subclusters_references,
+                                 z_score_filter = z_score_filter, restrict_to_DE_genes = restrict_to_DE_genes)
+    codes <- c(single = 0L, complete = 1L, average = 2L, mcquitty = 3L, ward.D = 4L, ward.D2 = 7L)
+    m <- infercnv_obj@expr.data
+    refs <- infercnv_obj@reference_grouped_cell_indices
+    obs <- infercnv_obj@observation_grouped_cell_indices
+    if (cluster_by_groups) {
+        tumor_groups <- c(obs, refs)
+    } else {
+        tumor_groups <- c(list(all_observations = unlist(obs, use.names = FALSE)), refs)
+    }
+    ok <- .icnv_enabled() && !isTRUE(restrict_to_DE_genes) && .icnv_ok(m) && nrow(m) >= 2 && is.character(hclust_method) &&
+        length(hclust_method) == 1 && hclust_method %in% names(codes) && is.character(partition_method) &&
+        length(partition_method) == 1 && partition_method %in% c("leiden", "qnorm", "pheight", "qgamma", "none") &&
+        all(lengths(tumor_groups) <= 65536)
+    if (!ok) return(call_orig())
+    leiden_method <- match.arg(leiden_method)
+    leiden_method_per_chr <- match.arg(leiden_method_per_chr)
+    leiden_function <- match.arg(leiden_function)
+    leiden_function_per_chr <- match.arg(leiden_function_per_chr)
+    futile.logger::flog.info(sprintf("define_signif_tumor_subclusters(p_val=%g", p_val))
+
+    ## the filter: keep = NULL (every gene) or the kept rows, 1-based
+    keep <- NULL
+    gene_order <- infercnv_obj@gene_order
+    if (z_score_filter > 0 && length(refs) > 0) {
+        flags <- .icnv_try(.Call("icnvR_zscore_outlier_genes", m, as.integer(unlist(refs, use.names = FALSE))), "z-score filter")
+        if (is.null(flags)) return(call_orig())
+        outliers <- which(flags)
+        keep <- seq_len(nrow(m))[-outliers]        # integer(0) when there is no outlier, as expr.data[-outliers, ] is
+        gene_order <- gene_order[-outliers, , drop = FALSE]
+    }
+    mk_hclust <- function(tr, cols) {
+        structure(list(merge = tr[[1]], height = tr[[2]], order = tr[[3]], labels = colnames(m)[cols], method = hclust_method,
+                       call = match.call(), dist.method = "euclidean"), class = "hclust")
+    }
+    trees_of <- function(lists) {
+        if (length(lists) == 0) return(list())
+        .icnv_try(.Call("icnvR_cluster_groups", m, if (is.null(keep)) NULL else as.integer(keep),
+                        lapply(lists, as.integer), codes[[hclust_method]]), "subcluster trees")
+    }
+
+    res <- list()
+    if (partition_method != "leiden") {
+        big <- names(tumor_groups)[lengths(tumor_groups) > 2]
+        trees <- trees_of(unname(tumor_groups[big]))
+        if (is.null(trees)) return(call_orig())
+        names(trees) <- big
+        for (tumor_group in names(tumor_groups)) {
+            futile.logger::flog.info(sprintf("define_signif_tumor_subclusters(), tumor: %s", tumor_group))
+            tumor_group_idx <- tumor_groups[[tumor_group]]
+            names(tumor_group_idx) <- colnames(m)[tumor_group_idx]
+            info <- list()
+            if (length(tumor_group_idx) > 2) {
+                hc <- mk_hclust(trees[[tumor_group]], tumor_group_idx)
+                info$hc <- hc
+                heights <- hc$height
+                if (partition_method == "pheight") {
+                    cut_height <- p_val * max(heights)
+                } else if (partition_method == "qnorm") {
+                    cut_height <- stats::qnorm(p = 1 - p_val, mean = mean(heights), sd = stats::sd(heights))
+                } else if (partition_method == "qgamma") {
+                    gamma_fit <- fitdistrplus::fitdist(heights, "gamma")
+                    cut_height <- stats::qgamma(p = 1 - p_val, shape = gamma_fit$estimate[1], rate = gamma_fit$estimate[2])
+                }
+                if (partition_method == "none") {
+                    grps <- stats::cutree(hc, k = 1)
+                } else {
+                    futile.logger::flog.info(sprintf("cut height based on p_val(%g) = %g and partition_method: %s", p_val,
+                                                     cut_height, partition_method))
+                    grps <- stats::cutree(hc, h = cut_height)
+                }
+                info$subclusters <- list()
+                s <- split(grps, grps)
+                futile.logger::flog.info(sprintf("cut tree into: %g groups", length(s)))
+                start_idx <- 1
+                for (g in names(s)) {
+                    split_subcluster <- paste0(tumor_group, "_s", g)
+                    futile.logger::flog.info(sprintf("-processing %s,%s", tumor_group, split_subcluster))
+                    end_idx <- start_idx + length(s[[g]]) - 1
+                    info$subclusters[[split_subcluster]] <- tumor_group_idx[hc$order[start_idx:end_idx]]
+                    start_idx <- end_idx + 1
+                }
+            } else {
+                info$hc <- NULL
+                info$subclusters[[paste0(tumor_group, "_s1")]] <- tumor_group_idx
+            }
+            res$hc[[tumor_group]] <- info$hc
+            res$subclusters[[tumor_group]] <- info$subclusters
+        }
+    } else {
+        ## every group's partition first, in group order (the RNG draws of the original's order)
+        expr_kept <- if (is.null(keep)) m else m[keep, , drop = FALSE]
+        parts <- list()
+        lists <- list()
+        for (tumor_group in names(tumor_groups)) {
+            futile.logger::flog.info(sprintf("define_signif_tumor_subclusters(), tumor: %s", tumor_group))
+            idx <- tumor_groups[[tumor_group]]
+            if (length(idx) < 3) {
+                futile.logger::flog.info(paste0("Too few cells in group ", tumor_group, " for any (sub)clustering. Keeping as is."))
+                next
+            }
+            if (k_nn >= length(idx)) {
+                futile.logger::flog.info(paste0("Less cells in group ", tumor_group, " than k_nn setting. Keeping as a single subcluster."))
+                lists[[length(lists) + 1]] <- idx
+                next
+            }
+            res_used <- if (identical(leiden_resolution, "auto")) (11.98 / length(idx))^(1 / 1.165) else leiden_resolution
+            if (identical(leiden_resolution, "auto"))
+                futile.logger::flog.info(sprintf("Setting auto leiden resolution for %s to %g", tumor_group, res_used))
+            tumor_expr_data <- expr_kept[, idx, drop = FALSE]
+            if (leiden_method == "PCA") {
+                partition <- infercnv:::.leiden_seurat_preprocess_routine(expr_data = tumor_expr_data, k_nn = k_nn,
+                                                                          resolution_parameter = res_used,
+                                                                          objective_function = leiden_function)
+            } else {
+                partition <- infercnv:::.leiden_simple_snn(tumor_expr_data, k_nn, res_used, leiden_function)
+            }
+            parts[[tumor_group]] <- partition
+            for (i in names(sort(table(partition), decreasing = TRUE))) {
+                w <- which(partition == i)
+                if (length(w) >= 2) lists[[length(lists) + 1]] <- idx[w]
+            }
+        }
+        trees <- trees_of(lists)
+        if (is.null(trees)) return(call_orig())
+        next_tree <- 0
+        for (tumor_group in names(tumor_groups)) {
+            idx <- tumor_groups[[tumor_group]]
+            names(idx) <- colnames(m)[idx]
+            if (length(idx) < 3) {
+                res$hc[[tumor_group]] <- NULL
+                res$subclusters[[tumor_group]] <- list()
+                res$subclusters[[tumor_group]][[paste0(tumor_group, "_s1")]] <- idx
+                next
+            }
+            if (k_nn >= length(idx)) {
+                next_tree <- next_tree + 1
+                res$subclusters[[tumor_group]] <- list()
+                res$subclusters[[tumor_group]][[tumor_group]] <- idx
+                res$hc[[tumor_group]] <- mk_hclust(trees[[next_tree]], idx)
+                next
+            }
+            partition <- parts[[tumor_group]]
+            subs <- list()
+            full <- NULL
+            for (i in names(sort(table(partition), decreasing = TRUE))) {
+                w <- which(partition == i)
+                subs[[paste(tumor_group, i, sep = "_s")]] <- idx[w]
+                if (length(w) >= 2) {
+                    next_tree <- next_tree + 1
+                    tmp <- ape::as.phylo(mk_hclust(trees[[next_tree]], idx[w]))
+                    if (is.null(full)) {
+                        full <- tmp
+                    } else {
+                        h1 <- phytools::get.rooted.tree.height(tmp)
+                        h2 <- phytools::get.rooted.tree.height(full)
+                        if (h1 == h2) {
+                            tmp$root.edge <- 1
+                            full$root.edge <- 1
+                        } else if (h1 > h2) {
+                            tmp$root.edge <- 1
+                            full$root.edge <- h1 - h2 + 1
+                        } else {
+                            tmp$root.edge <- h2 - h1 + 1
+                            full$root.edge <- 1
+                        }
+                        full <- tmp + full
+                    }
+                } else {
+                    full <- infercnv:::add_single_branch_to_phylo(full, colnames(m)[idx[w]])
+                }
+            }
+            res$hc[[tumor_group]] <- ape::as.hclust.phylo(full)
+            res$subclusters[[tumor_group]] <- subs
+        }
+    }
+    infercnv_obj@tumor_subclusters <- res
+
+    subclusters_per_chr <- NULL
+    if (per_chr_hmm_subclusters && partition_method == "leiden") {
+        if (!per_chr_hmm_subclusters_references) {
+            tumor_groups <- if (cluster_by_groups) obs else list(all_observations = unlist(obs, use.names = FALSE))
+        }
+        expr_kept <- if (is.null(keep)) m else m[keep, , drop = FALSE]
+        subclusters_per_chr <- infercnv:::.whole_dataset_leiden_subclustering_per_chr(
+            expr_data = expr_kept, tumor_groups = tumor_groups, chrs = gene_order$chr, k_nn = k_nn,
+            leiden_resolution = leiden_resolution_per_chr, leiden_method = leiden_method_per_chr,
+            leiden_function = leiden_function_per_chr)
+        if (!per_chr_hmm_subclusters_references) {
+            for (i in names(subclusters_per_chr)) subclusters_per_chr[[i]] <- c(subclusters_per_chr[[i]], refs)
+        }
+    }
+    if (!is.null(infercnv_obj@.hspike)) {
+        futile.logger::flog.info("-mirroring for hspike")
+        infercnv_obj@.hspike <- b200_define_signif_tumor_subclusters(infercnv_obj@.hspike, cluster_by_groups = TRUE,
+                                                                     partition_method = "none")[[1]]
+    }
+    list(infercnv_obj, subclusters_per_chr)
+}
+
 infercnvb200_install <- function() {
     fns <- c("subtract_ref_expr_from_obs", "smooth_by_chromosome", "center_cell_expr_across_chromosome",
              "predict_CNV_via_HMM_on_indiv_cells", "predict_CNV_via_HMM_on_tumor_subclusters",
@@ -785,6 +1015,7 @@ infercnvb200_install <- function() {
              "predict_CNV_via_HMM_on_tumor_subclusters_per_chr", "i3HMM_predict_CNV_via_HMM_on_tumor_subclusters",
              "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
              "mask_non_DE_genes_basic", "inferCNVBayesNet", "smooth_by_chromosome_coordinates",
+             "define_signif_tumor_subclusters",
              ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
              ".parameterize_random_cluster_heights_smoothed_trees")
     ns <- asNamespace("infercnv")

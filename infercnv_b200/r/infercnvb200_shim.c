@@ -580,6 +580,87 @@ SEXP icnvR_bayesnet(SEXP expr, SEXP genes, SEXP cells, SEXP pooled, SEXP mu, SEX
     return ans;
 }
 
+/* The z-score gene filter of define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:45-68): a logical vector of
+ * nrow(expr), TRUE where mean(abs(z)) >= 0.8 over the reference columns ref (1-based, unlist(reference_grouped_cell_indices)
+ * in that order).  The closure takes which() of it. */
+SEXP icnvR_zscore_outlier_genes(SEXP expr, SEXP ref) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int n = Rf_length(ref);
+    int32_t *idx = (int32_t *)malloc(sizeof(int32_t) * (size_t)(n > 0 ? n : 1));
+    uint8_t *out = (uint8_t *)malloc((size_t)(G > 0 ? G : 1));
+    int rc = ICNV_E_NOMEM;
+    if (idx && out) {
+        for (int i = 0; i < n; ++i) idx[i] = INTEGER(ref)[i] - 1;
+        rc = icnv_zscore_outlier_genes_f64(REAL(expr), G, C, idx, n, out);
+    }
+    free(idx);
+    SEXP ans = R_NilValue;
+    if (rc == 0) {
+        ans = PROTECT(Rf_allocVector(LGLSXP, (R_xlen_t)G));
+        for (int64_t g = 0; g < G; ++g) LOGICAL(ans)[g] = out[g] != 0;
+        UNPROTECT(1);
+    }
+    free(out);
+    fail_if(rc);
+    return ans;
+}
+
+/* hclust(parallelDist(t(expr[keep, g])), method) for every group g of `groups` (a list of 1-based column vectors) in one
+ * call: keep is NULL (every gene) or 1-based genes (integer(0): none).  Returns, per group, list(merge, height, order) or NULL
+ * for a group of fewer than 2 cells; the closure builds the "hclust" objects. */
+SEXP icnvR_cluster_groups(SEXP expr, SEXP keep, SEXP groups, SEXP method_code) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int32_t *off = NULL, *idx = NULL, *kp = NULL, *merge = NULL, *order = NULL;
+    double *height = NULL;
+    int n_grp = list_to_csr(groups, &off, &idx);
+    int64_t rows = 0, n_keep = Rf_isNull(keep) ? 0 : Rf_length(keep);
+    int rc = ICNV_E_NOMEM;
+    if (n_grp >= 0) {
+        for (int k = 0; k < n_grp; ++k) rows += off[k + 1] - off[k] >= 2 ? off[k + 1] - off[k] - 1 : 0;
+        kp = (int32_t *)malloc(sizeof(int32_t) * (size_t)(n_keep > 0 ? n_keep : 1));
+        merge = (int32_t *)malloc(sizeof(int32_t) * (size_t)(rows > 0 ? 2 * rows : 1));
+        height = (double *)malloc(sizeof(double) * (size_t)(rows > 0 ? rows : 1));
+        order = (int32_t *)malloc(sizeof(int32_t) * (size_t)(off[n_grp] > 0 ? off[n_grp] : 1));
+        if (kp && merge && height && order) {
+            for (int64_t i = 0; i < n_keep; ++i) kp[i] = INTEGER(keep)[i] - 1;
+            rc = icnv_cluster_groups_f64(REAL(expr), G, C, Rf_isNull(keep) ? NULL : kp, n_keep, off, idx, n_grp,
+                                         Rf_asInteger(method_code), merge, height, order);
+        }
+    }
+    SEXP ans = R_NilValue;
+    if (rc == 0) {
+        ans = PROTECT(Rf_allocVector(VECSXP, n_grp));
+        int64_t r = 0;
+        for (int k = 0; k < n_grp; ++k) {
+            const int64_t n = off[k + 1] - off[k];
+            if (n < 2) continue;
+            SEXP t = Rf_allocVector(VECSXP, 3);
+            SET_VECTOR_ELT(ans, k, t);
+            SEXP m = Rf_allocMatrix(INTSXP, (int)(n - 1), 2);
+            SET_VECTOR_ELT(t, 0, m);
+            memcpy(INTEGER(m), merge + 2 * r, sizeof(int32_t) * 2 * (size_t)(n - 1));
+            SEXP h = Rf_allocVector(REALSXP, (R_xlen_t)(n - 1));
+            SET_VECTOR_ELT(t, 1, h);
+            memcpy(REAL(h), height + r, sizeof(double) * (size_t)(n - 1));
+            SEXP o = Rf_allocVector(INTSXP, (R_xlen_t)n);
+            SET_VECTOR_ELT(t, 2, o);
+            memcpy(INTEGER(o), order + off[k], sizeof(int32_t) * (size_t)n);
+            r += n - 1;
+        }
+        UNPROTECT(1);
+    }
+    free(off);
+    free(idx);
+    free(kp);
+    free(merge);
+    free(height);
+    free(order);
+    fail_if(rc);
+    return ans;
+}
+
 SEXP icnvR_available(void) { return Rf_ScalarLogical(icnv_device_count() > 0 && icnv_init(-1) == 0); }
 
 static const R_CallMethodDef call_methods[] = {
@@ -600,6 +681,8 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_mask_non_de", (DL_FUNC)&icnvR_mask_non_de, 8},
     {"icnvR_bayesnet", (DL_FUNC)&icnvR_bayesnet, 10},
     {"icnvR_smooth_coordinates", (DL_FUNC)&icnvR_smooth_coordinates, 6},
+    {"icnvR_zscore_outlier_genes", (DL_FUNC)&icnvR_zscore_outlier_genes, 2},
+    {"icnvR_cluster_groups", (DL_FUNC)&icnvR_cluster_groups, 4},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

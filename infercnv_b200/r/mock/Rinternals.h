@@ -8,13 +8,16 @@ typedef void *(*DL_FUNC)(void);
 typedef struct _DllInfo DllInfo;
 typedef ptrdiff_t R_xlen_t;
 typedef struct { const char *name; DL_FUNC fun; int numArgs; } R_CallMethodDef;
+#define LGLSXP 10
 #define REALSXP 14
 #define INTSXP 13
 #define VECSXP 19
 #define FALSE 0
 extern SEXP R_DimSymbol;
+extern SEXP R_NilValue;
 SEXP Rf_getAttrib(SEXP, SEXP);
 int *INTEGER(SEXP);
+int *LOGICAL(SEXP);
 double *REAL(SEXP);
 int Rf_length(SEXP);
 R_xlen_t Rf_xlength(SEXP);

@@ -724,6 +724,118 @@ def parameterize_random_cluster_heights_smoothed_trees(expr_matrix, hclust_metho
     return {"h_obs": h_obs, "max_h": float(height.max()), "rand_max_height_dist": perm_max}
 
 
+def cutree(merge, height, k=None, h=None) -> np.ndarray:
+    """stats::cutree(tree, k = k, h = h) on a tree as hclust() returns it: the group (1-based) of every observation.  With h,
+    the merges of height <= h are applied (k = n + 1 - which.max(c(height, Inf) > h)); with k, the first n - k merges.  Groups
+    are numbered by first appearance in observation order."""
+    merge = np.asarray(merge)
+    n = merge.shape[0] + 1
+    if h is not None:
+        k = n - int(np.argmax(np.append(np.asarray(height, dtype=np.float64), np.inf) > h))
+    if k is None or not 1 <= k <= n:
+        raise ValueError(f"cutree: k = {k} for {n} observations")
+    lab = np.arange(n)                     # the observations' cluster representative, relabelled wholesale per merge
+    rep = np.zeros(n, dtype=np.int64)      # merge s + 1 -> its representative
+    for s in range(n - k):
+        a, b = (int(v) for v in merge[s])
+        ra = lab[-a - 1] if a < 0 else rep[a - 1]
+        rb = lab[-b - 1] if b < 0 else rep[b - 1]
+        lab[lab == ra] = rb
+        rep[s] = rb
+    _, first, inv = np.unique(lab, return_index=True, return_inverse=True)
+    return np.argsort(np.argsort(first))[inv] + 1
+
+
+def _assemble_subclusters(tumor_name: str, tumor_group_idx, order, grps) -> dict:
+    # .single_tumor_subclustering (R/inferCNV_tumor_subclusters.R:236-257): tumor_group_idx[hc$order] cut into consecutive
+    # runs, one per group of split(grps, grps) in group-id order, as long as that group
+    ordered = np.asarray(tumor_group_idx)[np.asarray(order) - 1]
+    ids, counts = np.unique(grps, return_counts=True)
+    ends = np.cumsum(counts)
+    return {f"{tumor_name}_s{g}": ordered[e - c:e] for g, c, e in zip(ids.tolist(), counts.tolist(), ends.tolist())}
+
+
+def _r_mean_sd(x):
+    # mean(x), sd(x) as R computes them: long-double sums with the refinement pass of mean() (summary.c, cov.c)
+    x = np.asarray(x, dtype=np.float64).astype(np.longdouble)
+    n = len(x)
+    m = np.cumsum(x)[-1] / n
+    m = m + np.cumsum(x - m)[-1] / n
+    d = x - m
+    return float(m), float(np.sqrt(np.float64(np.cumsum(d * d)[-1] / (n - 1))))
+
+
+def define_signif_tumor_subclusters(infercnv_obj: Infercnv, p_val: float = 0.1, k_nn: int = 20, leiden_method="PCA",
+                                    leiden_function="CPM", leiden_resolution="auto", leiden_method_per_chr="simple",
+                                    leiden_function_per_chr="modularity", leiden_resolution_per_chr=1,
+                                    hclust_method: str = "ward.D2", cluster_by_groups: bool = True,
+                                    partition_method: str = "leiden", per_chr_hmm_subclusters: bool = False,
+                                    per_chr_hmm_subclusters_references: bool = False, z_score_filter: float = 0.8,
+                                    restrict_to_DE_genes: bool = False):
+    """define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:2-177) for partition_method "none", "pheight" and
+    "qnorm": returns (infercnv_obj with tumor_subclusters = {"hc": {group: hclust dict or None}, "subclusters": {group:
+    {"<group>_s<id>": indices}}}, None), the hidden spike mirrored with partition_method "none".  The z-score gene filter
+    (icnv_zscore_outlier_genes_f64) and every group's tree (icnv_cluster_groups_f64) are two GPU calls; the cut heights and
+    cutree() are host arithmetic on the returned trees, as in R.  "qgamma" (fitdistrplus) and "leiden" (igraph's RNG) are not
+    on this path, nor is restrict_to_DE_genes."""
+    if partition_method in ("leiden", "qgamma"):
+        raise NotImplementedError(f"partition_method={partition_method!r} is not on the GPU path")
+    if partition_method not in ("none", "pheight", "qnorm"):
+        raise ValueError("Error, not recognizing parition_method")
+    if restrict_to_DE_genes:
+        raise NotImplementedError("restrict_to_DE_genes is not on the GPU path")
+    log.info("define_signif_tumor_subclusters(p_val=%g", p_val)
+    obj = copy.copy(infercnv_obj)
+    refs = obj.reference_grouped_cell_indices
+    obs = obj.observation_grouped_cell_indices
+    if cluster_by_groups:
+        tumor_groups = {**obs, **refs}
+    else:
+        allobs = np.concatenate([np.asarray(v) for v in obs.values()]) if obs else np.zeros(0, np.int64)
+        tumor_groups = {"all_observations": allobs, **refs}
+    keep = None
+    if z_score_filter > 0 and len(refs) > 0:
+        ref_cells = np.concatenate([np.asarray(v) for v in refs.values()])
+        outliers = api.zscore_outlier_genes(obj.expr_data, ref_cells)
+        keep = np.flatnonzero(~outliers)   # expr.data[-which(...), ]: no outlier gene keeps no gene at all
+        if not outliers.any():
+            keep = keep[:0]
+    names = list(tumor_groups)
+    treed = [g for g in names if len(tumor_groups[g]) > 2]
+    trees = dict(zip(treed, api.cluster_groups(obj.expr_data, [tumor_groups[g] for g in treed], method=hclust_method,
+                                               keep=keep)))
+    res = {"hc": {}, "subclusters": {}}
+    for g in names:
+        log.info("define_signif_tumor_subclusters(), tumor: %s", g)
+        idx = np.asarray(tumor_groups[g])
+        if g not in trees:
+            res["hc"][g] = None
+            res["subclusters"][g] = {f"{g}_s1": idx}
+            continue
+        merge, height, order = trees[g]
+        labels = [obj.cell_names[i] for i in idx] if obj.cell_names is not None else None
+        res["hc"][g] = {"merge": merge, "height": height, "order": order, "labels": labels, "method": hclust_method,
+                        "dist.method": "euclidean"}
+        if partition_method == "none":
+            grps = cutree(merge, height, k=1)
+        else:
+            if partition_method == "pheight":
+                cut = p_val * float(height.max())
+            else:
+                from scipy.stats import norm
+                mu, sigma = _r_mean_sd(height)
+                cut = float(norm.ppf(1 - p_val, loc=mu, scale=sigma))
+            log.info("cut height based on p_val(%g) = %g and partition_method: %s", p_val, cut, partition_method)
+            grps = cutree(merge, height, h=cut)
+        res["subclusters"][g] = _assemble_subclusters(g, idx, order, grps)
+        log.info("cut tree into: %d groups", len(res["subclusters"][g]))
+    obj.tumor_subclusters = res
+    if obj.hspike is not None:
+        log.info("-mirroring for hspike")
+        obj.hspike = define_signif_tumor_subclusters(obj.hspike, cluster_by_groups=True, partition_method="none")[0]
+    return obj, None
+
+
 def _tested_subclusters(infercnv_obj: Infercnv):
     """get_DE_genes_basic's loop (R/inferCNV_mask_non_DE.R:213-224): per observation group in order, its subclusters when
     they are a named list (a dict here), nothing when they are a plain index vector (R wraps it in an unnamed list)."""
