@@ -89,15 +89,13 @@ ICNV_API int64_t icnv_launch_count(void);
 
 /* HMM arithmetic.  mode 0: reference-order IEEE arithmetic for every sequence.  mode 1 (default): certified FP64 pass -
  * table emission + structured recursion, every arg-max margin checked, and each sequence whose smallest margin is below
- * 1e-7 recomputed in mode-0 arithmetic.  mode 2 (option, measured slower on the benchmark data): a single-precision pass
- * first, certified by the margins along the returned path only; what it cannot certify goes through the mode-1 pass, what
- * that cannot certify through mode 0.  The state calls are the same in all modes.  Also settable with the environment
- * variable ICNV_HMM_MODE (read at icnv_init). */
+ * 1e-7 recomputed in mode-0 arithmetic.  The state calls are the same in both modes.  Any other mode is refused with
+ * ICNV_E_BAD_ARG.  Also settable with the environment variable ICNV_HMM_MODE (read at icnv_init: "0" or "e..." selects
+ * mode 0, anything else mode 1). */
 ICNV_API int icnv_set_hmm_mode(int mode);
 /* Number of sequences the last Viterbi call recomputed in reference-order arithmetic (syncs). */
 ICNV_API int64_t icnv_hmm_rerun_count(void);
-/* Number of sequences the single-precision pass (mode 2) of the last Viterbi call could not certify and handed to the FP64
- * pass (syncs); 0 in modes 0 and 1. */
+/* Always 0: no HMM mode hands sequences to a second pass.  Kept so that existing callers still link. */
 ICNV_API int64_t icnv_hmm_second_pass_count(void);
 
 /* ---- host-pointer entry points (what the R shim binds) ---------------------------------------- */

@@ -85,10 +85,9 @@ def launch_count() -> int:
 
 
 def set_hmm_mode(mode) -> None:
-    """0 / "exact": reference-order arithmetic; 1 / "fast" / "fast64": certified FP64 pass (default); 2 / "fast32": a
-    single-precision pass certified by per-path margins first, then the FP64 pass for what it cannot certify (measured slower
-    on the benchmark data, kept as an option).  What no pass certifies is recomputed in reference-order arithmetic."""
-    m = {"exact": 0, "fast": 1, "fast64": 1, "fast32": 2}.get(mode, mode)
+    """0 / "exact": reference-order arithmetic; 1 / "fast" / "fast64": certified FP64 pass (default).  What the certified
+    pass cannot certify is recomputed in reference-order arithmetic."""
+    m = {"exact": 0, "fast": 1, "fast64": 1}.get(mode, mode)
     _lib.check(_lib.load().icnv_set_hmm_mode(int(m)))
 
 
@@ -105,7 +104,7 @@ def hmm_rerun_count() -> int:
 
 
 def hmm_second_pass_count() -> int:
-    """sequences the single-precision pass of the last Viterbi call handed to the FP64 pass"""
+    """always 0: no HMM mode hands sequences to a second pass"""
     return int(_lib.load().icnv_hmm_second_pass_count())
 
 

@@ -376,21 +376,17 @@ static int env_int(const char *name, int dflt, bool *set = nullptr) {
 // default is reported, so a stray variable in a user's shell cannot silently change which kernel runs.
 static void read_options(Ctx &c, bool verbose) {
     bool set;
-    if (const char *e = getenv("ICNV_HMM_MODE")) c.hmm_mode = (e[0] == '0' || e[0] == 'e') ? 0 : (e[0] == '2' ? 2 : 1);
+    if (const char *e = getenv("ICNV_HMM_MODE")) c.hmm_mode = (e[0] == '0' || e[0] == 'e') ? 0 : 1;
     c.opt_cell_kernel = env_int("ICNV_CELL_KERNEL", 0);
     c.opt_cell_nt = env_int("ICNV_CELL_NT", 0);
     c.opt_cell_variant = env_int("ICNV_CELL_VARIANT", -1);
     c.opt_cell_padq = env_int("ICNV_CELL_PADQ", 1);
     c.opt_cell_lfix = env_int("ICNV_CELL_LFIX", 1);
-    c.opt_vfast_warps = env_int("ICNV_VFAST_WARPS", 0);
-    c.opt_mf_kernel = env_int("ICNV_MF_KERNEL", -1);
-    c.opt_mf_list32 = env_int("ICNV_MF_LIST32", 0);
-    c.opt_vit_evict = env_int("ICNV_VIT_EVICT", 2);
     c.opt_slab_cells = env_int("ICNV_SLAB_CELLS", 0, &set);
     if (c.opt_slab_cells < 32 || c.opt_slab_cells > 65536) c.opt_slab_cells = 0;
     if (!verbose) return;
     static const char *names[] = {"ICNV_HMM_MODE", "ICNV_CELL_KERNEL", "ICNV_CELL_NT", "ICNV_CELL_VARIANT", "ICNV_CELL_PADQ",
-                                  "ICNV_CELL_LFIX", "ICNV_VFAST_WARPS", "ICNV_MF_KERNEL", "ICNV_MF_LIST32", "ICNV_SLAB_CELLS", "ICNV_VIT_EVICT"};
+                                  "ICNV_CELL_LFIX", "ICNV_SLAB_CELLS"};
     for (const char *n : names)
         if (const char *e = getenv(n)) fprintf(stderr, "[infercnv_b200] non-default tuning switch %s=%s (read once at icnv_init)\n", n, e);
 }
@@ -422,13 +418,10 @@ static int init_slot(int slot, int device) {
     c.device = device;
     c.launches = 0;
     c.table_uploaded = false;
-    c.table32_uploaded = false;
     c.math_tables_uploaded = false;
     c.up_segs.clear();
     c.up_items.clear();
     c.hmm_list_count = nullptr;
-    c.hmm_seq_counts = nullptr;
-    c.hmm_seq_k = 0;
     c.rg_n = 0;
     read_options(c, slot == 0);
     c.ready = true;

@@ -50,8 +50,6 @@ enum ScratchSlot {
     SLOT_RG_REC,                      // region records of the last call (kept until fetched)
     SLOT_VIT_ITEMS,                   // chromosome work items of the Viterbi launch (cached: Ctx::up_items)
     SLOT_MF_PRE,                      // median filter: range of the matrix and the value sample of its pre-pass
-    SLOT_TABLE32,                     // single-precision emission table
-    SLOT_SEQ,                         // per-chromosome lists of the sequences for the FP64 second pass
     SLOT_KNN,                         // k nearest neighbours: per-split partial lists and the non-finite flag
     SLOT_COUNT
 };
@@ -67,12 +65,10 @@ struct Ctx {
     void *slot_ptr[SLOT_COUNT] = {};
     size_t slot_bytes[SLOT_COUNT] = {};
     std::atomic<int64_t> launches{0};
-    int hmm_mode = 1;                 // 0 reference-order arithmetic, 1 certified FP64 pass (default), 2 FP32 pass first (per-path margins; measured slower)
-    bool table_uploaded = false, table32_uploaded = false;
+    int hmm_mode = 1;                 // 0 reference-order arithmetic, 1 certified FP64 pass (default)
+    bool table_uploaded = false;
     bool math_tables_uploaded = false;
     unsigned int *hmm_list_count = nullptr;  // device counter of the last Viterbi call's re-run list
-    unsigned int *hmm_seq_counts = nullptr;  // per-chromosome counts of the sequences the single-precision pass handed on
-    int hmm_seq_k = 0;
     int64_t rg_n = 0;                 // number of region records held in SLOT_RG_REC
     // what the small per-launch tables (thread segments of the cell pipeline, chromosome items of the Viterbi) held when
     // they were last uploaded: an unchanged table is not copied again, so the slab loop of the host pipeline enqueues
@@ -84,7 +80,6 @@ struct Ctx {
     size_t pin_bytes[6] = {};
     // tuning switches, read from the environment ONCE in icnv_init (never at launch time); -1 / 0 = library default
     int opt_cell_kernel = 0, opt_cell_nt = 0, opt_cell_variant = -1, opt_cell_padq = 1, opt_cell_lfix = 1;
-    int opt_vfast_warps = 0, opt_mf_kernel = -1, opt_mf_list32 = 0, opt_vit_evict = 2;
     long opt_slab_cells = 0;
     // the cell-pipeline instantiation the last icnv_dev_cell_pipeline_f64 call launched: family (3 / 4), NT, MINB, PADQ, LFIX,
     // slice length L; all zero when that call launched nothing (refused, or no columns)

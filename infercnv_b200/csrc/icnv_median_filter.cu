@@ -5,10 +5,11 @@
 // as in the reference (noise_reduction.R:102-106: half_window + 1).  Even-count windows average
 // the two middle values (median.default).  Reads the un-filtered input throughout.
 //
-// One thread per output element.  Window sizes 3..9 (radius 2..5) run median_filter_select_kernel: the tile's halo is
-// staged in shared memory and every thread selects its window's median by counting (icnv_median_select.cuh - no
-// data-dependent partitioning, so the lanes of a warp stay together).  Other window sizes use the generic kernel
-// below (in-place Wirth selection over a private index array).
+// One thread per output element.  Window sizes 3, 5 and 9 (radius 2, 3, 5) run median_filter_select_kernel: the tile's
+// halo is staged in shared memory and every thread selects its window's median by counting (icnv_median_select.cuh - no
+// data-dependent partitioning, so the lanes of a warp stay together).  Window size 7 (radius 4, the reference's default)
+// runs the shared-merge kernel further down.  Larger window sizes use the generic kernel below (in-place Wirth selection
+// over a private index array).
 #include <cfloat>
 #include <cmath>
 #include <algorithm>
@@ -37,7 +38,6 @@ struct MfParams {
     const MfTile *cell_tiles; // gridDim.x entries
     int r;
     int *err_flag;
-    int use_net;              // radius 4 only: full windows by the key network (window_median_net81), 0 = counting selection
     // shared-merge kernel: the matrix' range (keys quantise over it) and its dominant value (NaN: none), found before the launch
     double vmin, vmax, mode;
     double scale;             // (2^24 - 3) / (vmax - vmin), 0 if the matrix is constant
@@ -125,16 +125,13 @@ __global__ void __launch_bounds__(MF_NT) median_filter_kernel(const MfParams p) 
 // are consecutive doubles (no bank conflicts) and the per-thread tap lists interleave at 2-byte granularity.
 constexpr int MS_TI = 32, MS_TJ = 8, MS_NT = MS_TI * MS_TJ;
 
-// NET (radius 4 only): full windows go through the key network (window_median_net81, ~160 registers per thread); a separate
-// instance, so that the counting-selection kernel keeps its 64 registers and four CTAs per SM.
-template <int R, typename ListT = unsigned short, bool NET = false>
-__global__ void __launch_bounds__(MS_NT, NET ? 2 : 0) median_filter_select_kernel(const MfParams p) {
+template <int R>
+__global__ void __launch_bounds__(MS_NT) median_filter_select_kernel(const MfParams p) {
     extern __shared__ __align__(16) unsigned char mf_smem[];
     constexpr int D = 2 * R + 1, HR = MS_TI + 2 * R, HC = MS_TJ + 2 * R;
     double *halo = reinterpret_cast<double *>(mf_smem);          // +inf outside the block: never counted
     double *halo0 = halo + HR * HC;                              // 0 outside the block: for the window moments
-    ListT *list = reinterpret_cast<ListT *>(halo0 + HR * HC);   // [D*D][MS_NT] tap offsets
-    float *kf = reinterpret_cast<float *>(list + (size_t)D * D * MS_NT);   // use_net: single-precision keys of the halo
+    unsigned short *list = reinterpret_cast<unsigned short *>(halo0 + HR * HC);   // [D*D][MS_NT] tap offsets
     const MfTile gt = p.gene_tiles[blockIdx.y];
     const MfTile ct = p.cell_tiles[blockIdx.x];
     const int hi0 = gt.start - R, hj0 = ct.start - R;
@@ -150,25 +147,15 @@ __global__ void __launch_bounds__(MS_NT, NET ? 2 : 0) median_filter_select_kerne
         }
         halo[e] = v;
         halo0[e] = v0;
-        if (NET) kf[e] = (float)v;
     }
     __syncthreads();
     const int ti = threadIdx.x % MS_TI, tj = threadIdx.x / MS_TI;
-    // a tile whose every window is a full (2R+1)^2 one (no tap outside the chromosome / index-list block): CTA-uniform
-    const bool full_tile = gt.len == MS_TI && ct.len == MS_TJ && gt.start - R >= gt.lo && gt.start + MS_TI + R <= gt.hi &&
-                           ct.start - R >= ct.lo && ct.start + MS_TJ + R <= ct.hi;
     if (ti < gt.len && tj < ct.len) {
         const int i = gt.start + ti, j = ct.start + tj;
-        double med;
-        if (NET && full_tile) {
-            med = window_median_net81<ListT>(halo, halo0, kf, HR, tj * HR + ti, list + threadIdx.x, MS_NT);
-        } else {
-            const int xa = max(gt.lo, i - R), xb = min(gt.hi - 1, i + R);
-            const int ya = max(ct.lo, j - R), yb = min(ct.hi - 1, j + R);
-            const int n = (xb - xa + 1) * (yb - ya + 1);
-            med = window_median<R, ListT>(halo, halo0, HR, tj * HR + ti, list + threadIdx.x, MS_NT, n);
-        }
-        p.Y[i + p.G * (int64_t)p.cells[j]] = med;
+        const int xa = max(gt.lo, i - R), xb = min(gt.hi - 1, i + R);
+        const int ya = max(ct.lo, j - R), yb = min(ct.hi - 1, j + R);
+        const int n = (xb - xa + 1) * (yb - ya + 1);
+        p.Y[i + p.G * (int64_t)p.cells[j]] = window_median<R>(halo, halo0, HR, tj * HR + ti, list + threadIdx.x, MS_NT, n);
     }
     if (bad && p.err_flag) atomicExch(p.err_flag, 1);
 }
@@ -230,32 +217,16 @@ constexpr unsigned MM_LOW = 0u, MM_HIGH = 0xffffffffu;
 
 // TY = outputs per tile along the index list.  Halo rows 0 .. TY+9 (row r = list position y0 - 5 + r; rows 1 .. TY+8 are used);
 // P lists: rows (2t, 2t+1), t = 1 .. TY/2+3; Q lists: P[q] + P[q+1].
-// DH = false: the tile keeps no copy of the halo's doubles; the few that are needed (the median's own value, the members of a
-// tied key cell) are read from the matrix again (L2), through the tile's table of column offsets.
-constexpr size_t mm_smem_bytes(int TY, bool DH = true) {
-    return (DH ? sizeof(double) * (size_t)(TY + 10) * MM_HX : 0) + sizeof(unsigned) * (size_t)(TY + 10) * MM_HX +
+constexpr size_t mm_smem_bytes(int TY) {
+    return sizeof(double) * (size_t)(TY + 10) * MM_HX + sizeof(unsigned) * (size_t)(TY + 10) * MM_HX +
            sizeof(unsigned) * (size_t)(TY + 10) * 9 * MM_TX + sizeof(unsigned) * (size_t)(TY / 2 + 3) * MM_TX * MM_PW +
            sizeof(unsigned) * (size_t)(TY / 2 + 2) * MM_TX * MM_QW + 96 * sizeof(double);
 }
 
 // The value of real rank `rho` (1-based, among the window's taps inside the block) when the key at that rank has the
 // quantised value Q: every tap below the cell ranks below it, so the answer is the (rho - #below)-th smallest double of the
-// cell.  (x0, r0): halo coordinates of the window's first tap.
-// the halo's doubles: from the tile's shared copy, or (no copy kept) from the matrix through the tile's column-offset table
-template <bool DH>
-struct MmVals {
-    const double *Dh;            // [ROWS][HX] (DH)
-    const double *X;
-    const long long *rowoff;     // [ROWS] column offset of each halo row (!DH)
-    long long hi0;               // gene of halo column 0
-    __device__ __forceinline__ double operator()(int r, int hx) const {
-        if constexpr (DH) return Dh[r * MM_HX + hx];
-        else return X[hi0 + hx + rowoff[r]];
-    }
-};
-
-template <bool DH>
-__device__ __noinline__ double mm_exact_rank(const unsigned *__restrict__ Kh, const MmVals<DH> Dv, int x0, int r0, unsigned Q, int rho) {
+// cell.  (x0, r0): halo coordinates of the window's first tap; Dh: the tile's halo values, [ROWS][HX].
+__device__ __noinline__ double mm_exact_rank(const unsigned *__restrict__ Kh, const double *__restrict__ Dh, int x0, int r0, unsigned Q, int rho) {
     int below = 0, g = 0;
     double dmin = INFINITY, dmax = -INFINITY;
     for (int r = 0; r < 9; ++r)
@@ -265,7 +236,7 @@ __device__ __noinline__ double mm_exact_rank(const unsigned *__restrict__ Kh, co
             const unsigned q = key >> 8;
             below += (q < Q) ? 1 : 0;
             if (q == Q) {
-                const double d = Dv(r0 + r, x0 + c);
+                const double d = Dh[(r0 + r) * MM_HX + x0 + c];
                 ++g;
                 dmin = d < dmin ? d : dmin;
                 dmax = d > dmax ? d : dmax;
@@ -278,13 +249,13 @@ __device__ __noinline__ double mm_exact_rank(const unsigned *__restrict__ Kh, co
         for (int c = 0; c < 9; ++c) {
             const unsigned key = Kh[(r0 + r) * MM_HX + x0 + c];
             if (key == MM_LOW || key == MM_HIGH || (key >> 8) != Q) continue;
-            const double d = Dv(r0 + r, x0 + c);
+            const double d = Dh[(r0 + r) * MM_HX + x0 + c];
             int lt = 0, eq = 0;
             for (int r2 = 0; r2 < 9; ++r2)
                 for (int c2 = 0; c2 < 9; ++c2) {
                     const unsigned k2 = Kh[(r0 + r2) * MM_HX + x0 + c2];
                     if (k2 == MM_LOW || k2 == MM_HIGH || (k2 >> 8) != Q) continue;
-                    const double d2 = Dv(r0 + r2, x0 + c2);
+                    const double d2 = Dh[(r0 + r2) * MM_HX + x0 + c2];
                     lt += (d2 < d) ? 1 : 0;
                     eq += (d2 == d) ? 1 : 0;
                 }
@@ -294,19 +265,18 @@ __device__ __noinline__ double mm_exact_rank(const unsigned *__restrict__ Kh, co
 }
 
 // the double behind a key of the window whose first tap is (x0, r0): the tag holds the tap's halo coordinates mod 16
-template <bool DH>
-__device__ __forceinline__ double mm_value_of(const MmVals<DH> &Dv, unsigned key, int x0, int r0) {
+__device__ __forceinline__ double mm_value_of(const double *Dh, unsigned key, int x0, int r0) {
     const int tx = (int)((key >> 4) & 15u), ty = (int)(key & 15u);
     const int hx = x0 + ((tx - x0) & 15), r = r0 + ((ty - r0) & 15);
-    return Dv(r, hx);
+    return Dh[r * MM_HX + hx];
 }
 
-template <int MM_TY, int MM_NW, int MINB, bool DH = true>
+template <int MM_TY, int MM_NW, int MINB>
 __global__ void __launch_bounds__(MM_NW * 32, MINB) median_filter_merge_kernel(const MfParams p) {
     constexpr int MM_ROWS = MM_TY + 10, MM_NT = MM_NW * 32, MM_NP = MM_TY / 2 + 3, MM_NQ = MM_TY / 2 + 2;
     extern __shared__ __align__(16) unsigned char mf_smem[];
-    double *Dh = reinterpret_cast<double *>(mf_smem);                         // [ROWS][HX] values (0 outside the block); DH only
-    double *redd = Dh + (DH ? MM_ROWS * MM_HX : 0);                           // [96] flags, table of the halo rows' column offsets
+    double *Dh = reinterpret_cast<double *>(mf_smem);                         // [ROWS][HX] values (0 outside the block)
+    double *redd = Dh + MM_ROWS * MM_HX;                                      // [96] flags
     unsigned *Kh = reinterpret_cast<unsigned *>(redd + 96);                   // [ROWS][HX] keys
     unsigned *Rs = Kh + MM_ROWS * MM_HX;                                      // [ROWS][9][TX] sorted runs
     unsigned *Ps = Rs + (size_t)MM_ROWS * 9 * MM_TX;                          // [NP][TX][PW]
@@ -333,8 +303,6 @@ __global__ void __launch_bounds__(MM_NW * 32, MINB) median_filter_merge_kernel(c
     const unsigned qM = quant(M);
     int *flags = reinterpret_cast<int *>(redd);
     if (tid == 0) flags[0] = 0;
-    long long *rowoff = reinterpret_cast<long long *>(redd) + 8;   // [MM_ROWS] <= 42 of the 96 scratch doubles (DH = false)
-    const MmVals<DH> Dv{Dh, p.X, rowoff, (long long)hi0};
     // a tap's value -> its key and the two halo arrays
     auto put = [&](int r, int hx, bool in, double v) {
         unsigned key = ((hx + r) & 1) ? MM_HIGH : MM_LOW;
@@ -344,7 +312,7 @@ __global__ void __launch_bounds__(MM_NW * 32, MINB) median_filter_merge_kernel(c
             dirty |= (q == qM) && (v != M);
             key = (q << 8) | (unsigned)((hx & 15) << 4) | (unsigned)(r & 15);
         }
-        if (DH) Dh[r * MM_HX + hx] = in ? v : 0.0;
+        Dh[r * MM_HX + hx] = in ? v : 0.0;
         Kh[r * MM_HX + hx] = key;
     };
     // every global load of the tile is issued before the first one is used: first the column offsets (G * cell, a table the
@@ -360,7 +328,6 @@ __global__ void __launch_bounds__(MM_NW * 32, MINB) median_filter_merge_kernel(c
         const int jj = hj0 + r;
         rin[i] = r < MM_ROWS && jj >= ct.lo && jj < ct.hi && r >= 1 && r <= MM_TY + 8;
         rb[i] = rin[i] ? p.coloff[jj] : 0ll;
-        if (!DH && i < RPW && lane == 0 && r < MM_ROWS) rowoff[r] = rb[i];   // read again in S3 only (two barriers later)
     }
     double tv[RPW + TPW];
 #pragma unroll
@@ -474,14 +441,14 @@ __global__ void __launch_bounds__(MM_NW * 32, MINB) median_filter_merge_kernel(c
                 auto value_at = [&](int ki, int rk) -> double {
                     const unsigned Qc = s[ki] >> 8;
                     const bool tl = (s[ki - 1] >> 8) == Qc, th = (s[ki + 1] >> 8) == Qc;
-                    if (!tl && !th) return mm_value_of(Dv, s[ki], x0, r0);
+                    if (!tl && !th) return mm_value_of(Dh, s[ki], x0, r0);
                     if (Qc == qM && mode_clean) return M;
                     int lo = ki, hi = ki;
                     while (lo > 0 && (s[lo - 1] >> 8) == Qc) --lo;
                     while (hi < 4 && (s[hi + 1] >> 8) == Qc) ++hi;
-                    if (lo == 0 || hi == 4 || hi - lo > 2) return mm_exact_rank(Kh, Dv, x0, r0, Qc, rk);
-                    double d0 = mm_value_of(Dv, s[lo], x0, r0), d1 = mm_value_of(Dv, s[lo + 1], x0, r0);
-                    double d2 = (hi - lo == 2) ? mm_value_of(Dv, s[lo + 2], x0, r0) : INFINITY;
+                    if (lo == 0 || hi == 4 || hi - lo > 2) return mm_exact_rank(Kh, Dh, x0, r0, Qc, rk);
+                    double d0 = mm_value_of(Dh, s[lo], x0, r0), d1 = mm_value_of(Dh, s[lo + 1], x0, r0);
+                    double d2 = (hi - lo == 2) ? mm_value_of(Dh, s[lo + 2], x0, r0) : INFINITY;
                     mf_cswap(d0, d1);
                     mf_cswap(d1, d2);
                     mf_cswap(d0, d1);
@@ -520,27 +487,16 @@ extern "C" int icnv_dev_median_filter_f64(const double *X, double *Y, int64_t G,
         return set_error(ICNV_E_BAD_ARG, "window_size must be an odd number >= 3 (noise_reduction.R:48-50)");
     const int r = (window_size + 1) / 2;
     const int W = (2 * r + 1) * (2 * r + 1);
-    bool select_kernel = (r >= 2 && r <= 5);
-    int use_net = 0;
-    if (c.opt_mf_kernel >= 0) {   // ICNV_MF_KERNEL, read once in icnv_init: 0 generic kernel; 2 key network for full 9 x 9 windows (A/B runs)
-        select_kernel = select_kernel && (c.opt_mf_kernel != 0);
-        use_net = (c.opt_mf_kernel == 2 && r == 4) ? 1 : 0;
-    }
-    // window_size 7 (radius 4): the shared-merge kernel; ICNV_MF_KERNEL=1 (read at icnv_init) keeps the counting selection
-    // (default and ICNV_MF_KERNEL=4: tiles of 12 list positions, two 256-thread CTAs per SM; 3: tiles of 32, one 512-thread CTA)
-    // (5: tiles of 16, two 320-thread CTAs per SM, no shared copy of the halo's doubles)
-    const int mm_ty = (c.opt_mf_kernel == 3) ? 32 : (c.opt_mf_kernel == 5 ? 16 : 12);
-    const int mm_nw = (c.opt_mf_kernel == 3) ? 16 : (c.opt_mf_kernel == 5 ? 10 : 8);
-    const bool mm_dh = c.opt_mf_kernel != 5;
-    const bool merge_kernel = (r == 4) && (c.opt_mf_kernel < 0 || c.opt_mf_kernel >= 3) && mm_smem_bytes(mm_ty, mm_dh) <= (size_t)c.smem_optin;
+    // window_size 7 (radius 4): the shared-merge kernel, tiles of 12 list positions, two 256-thread CTAs per SM; the other
+    // windows up to radius 5: the counting selection; larger ones: the generic kernel
+    constexpr int mm_ty = 12, mm_nw = 8;
+    const bool merge_kernel = r == 4;
+    const bool select_kernel = !merge_kernel && r >= 2 && r <= 5;
     const int TI = merge_kernel ? MM_TX : (select_kernel ? MS_TI : MF_TI), TJ = merge_kernel ? mm_ty : (select_kernel ? MS_TJ : MF_TJ);
     const int NT = merge_kernel ? mm_nw * 32 : TI * TJ;
-    bool list32 = false;
-    if (c.opt_mf_list32) list32 = select_kernel;   // diagnostic (ICNV_MF_LIST32 at icnv_init)
-    const size_t smem = merge_kernel ? mm_smem_bytes(mm_ty, mm_dh)
+    const size_t smem = merge_kernel ? mm_smem_bytes(mm_ty)
                                      : sizeof(double) * (size_t)(TI + 2 * r) * (size_t)(TJ + 2 * r) * (select_kernel ? 2 : 1) +
-                                           (list32 ? sizeof(unsigned) : sizeof(unsigned short)) * (size_t)W * (size_t)NT +
-                                           (use_net ? sizeof(float) * (size_t)(TI + 2 * r) * (size_t)(TJ + 2 * r) : 0);
+                                           sizeof(unsigned short) * (size_t)W * (size_t)NT;
     if (smem > (size_t)c.smem_optin || (TI + 2 * r) * (TJ + 2 * r) > 65535)
         return set_error(ICNV_E_UNSUPPORTED, "window_size %d needs %zu B of shared memory per CTA", window_size, smem);
     cudaStream_t st = pick_stream(stream);
@@ -607,7 +563,7 @@ extern "C" int icnv_dev_median_filter_f64(const double *X, double *Y, int64_t G,
     }
     ICNV_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
     ICNV_CUDA(cudaStreamSynchronize(st));  // tile tables are stack-lifetime host buffers
-    MfParams p{X, Y, G, d_cells, d_gt, d_ct, r, d_flag, use_net, 0.0, 0.0, 0.0, 0.0, d_coloff};
+    MfParams p{X, Y, G, d_cells, d_gt, d_ct, r, d_flag, 0.0, 0.0, 0.0, 0.0, d_coloff};
     if (merge_kernel) {
         // range of the matrix + a sample of its values (the dominant value is the most frequent one of the sample, if any
         // value takes >= 0.5 % of it)
@@ -657,17 +613,10 @@ extern "C" int icnv_dev_median_filter_f64(const double *X, double *Y, int64_t G,
         return ICNV_OK;
     };
     int lrc;
-    if (list32) use_net = 0;
-    if (merge_kernel)
-        lrc = (mm_ty == 12) ? launch(median_filter_merge_kernel<12, 8, 2>)
-                            : (mm_ty == 16 ? launch(median_filter_merge_kernel<16, 10, 2, false>) : launch(median_filter_merge_kernel<32, 16, 1>));
+    if (merge_kernel) lrc = launch(median_filter_merge_kernel<mm_ty, mm_nw, 2>);
     else if (!select_kernel) lrc = launch(median_filter_kernel);
-    else if (list32 && r == 5) lrc = launch(median_filter_select_kernel<5, unsigned>);
-    else if (list32 && r == 4) lrc = launch(median_filter_select_kernel<4, unsigned>);
     else if (r == 2) lrc = launch(median_filter_select_kernel<2>);
     else if (r == 3) lrc = launch(median_filter_select_kernel<3>);
-    else if (r == 4 && use_net) lrc = launch(median_filter_select_kernel<4, unsigned short, true>);
-    else if (r == 4) lrc = launch(median_filter_select_kernel<4>);
     else lrc = launch(median_filter_select_kernel<5>);
     if (lrc) return lrc;
     ICNV_CHECK_LAUNCH("median_filter_kernel");

@@ -80,8 +80,8 @@ ICNV_HD void mf_sort16(double (&c)[16]) {
 // n: number of taps inside the block (>= 1).  stats (optional): [0] += list rounds, [1] += second build passes.
 constexpr int MF_CAND = 16;   // candidates ordered directly at the end
 
-template <int R, typename ListT = unsigned short>
-ICNV_HD double window_median(const double *halo, const double *halo0, int HR, int idx0, ListT *list, int ls, int n,
+template <int R>
+ICNV_HD double window_median(const double *halo, const double *halo0, int HR, int idx0, unsigned short *list, int ls, int n,
                              unsigned *stats = nullptr) {
     constexpr int D = 2 * R + 1;
     const int k = (n - 1) >> 1;
@@ -125,7 +125,7 @@ ICNV_HD double window_median(const double *halo, const double *halo0, int HR, in
                 const bool inside = !below && (v <= bhi);
                 c_lo += below ? 1 : 0;
                 if (inside) {
-                    list[cnt * ls] = (ListT)(dj * HR + di);
+                    list[cnt * ls] = (unsigned short)(dj * HR + di);
                     ++cnt;
                 }
             }
@@ -242,7 +242,7 @@ ICNV_HD double window_median(const double *halo, const double *halo0, int HR, in
     if (!have_result) {
         int c = 0;
         for (int t = 0; t < cnt; ++t) {   // in place: the write position never passes the read position
-            const ListT e = list[t * ls];
+            const unsigned short e = list[t * ls];
             const double v = w[e];
             if (v > lo && v <= hi) {
                 list[c * ls] = e;
@@ -276,61 +276,6 @@ ICNV_HD double window_median(const double *halo, const double *halo0, int HR, in
         next = mn;
     }
     return (result + next) * 0.5;
-}
-
-// ---- full 9 x 9 windows (radius 4, the default apply_median_filtering window of 7: noise_reduction.R:102-106) by a
-// comparator network on single-precision KEYS ------------------------------------------------------------------------------
-// (float)v is a monotone map, so the order of the keys never contradicts the order of the values: the key at rank 40 of the
-// 81 keys belongs to the median itself unless several distinct values share that key.  The network (icnv_median_net81.inc,
-// generated and checked by tools/gen_median_network.py: Batcher's odd-even merge sort pruned to what rank 40 depends on,
-// 702 comparators = 1324 min / max instructions on registers, no shared-memory traffic, no data-dependent control flow)
-// finds that key; one more pass over the keys finds its tap.  Ties in the key are exact when the tied values are identical
-// (de-noised matrices: a run of one constant); distinct values under one key (closer than 6e-8 relative, around the median)
-// go to window_median.  kf: the tile's keys, laid out like halo.
-ICNV_HD float mf_net81_median(float (&k)[81]) {
-#define CS(a, b) { const float lo_ = fminf(k[a], k[b]), hi_ = fmaxf(k[a], k[b]); k[a] = lo_; k[b] = hi_; }
-#define MN(a, b) k[a] = fminf(k[a], k[b]);
-#define MX(a, b) k[b] = fmaxf(k[a], k[b]);
-#include "icnv_median_net81.inc"
-#undef CS
-#undef MN
-#undef MX
-    return k[40];
-}
-
-template <typename ListT = unsigned short>
-ICNV_HD double window_median_net81(const double *halo, const double *halo0, const float *kf, int HR, int idx0, ListT *list, int ls,
-                                   unsigned *stats = nullptr) {
-    constexpr int D = 9;
-    const float *q = kf + idx0;
-    float k[D * D];
-#pragma unroll
-    for (int dj = 0; dj < D; ++dj)
-#pragma unroll
-        for (int di = 0; di < D; ++di) k[dj * D + di] = q[dj * HR + di];
-    const float m = mf_net81_median(k);
-    int c_eq = 0, tap = 0;
-#pragma unroll
-    for (int dj = 0; dj < D; ++dj)
-#pragma unroll
-        for (int di = 0; di < D; ++di) {
-            const bool e = q[dj * HR + di] == m;
-            c_eq += e ? 1 : 0;
-            tap = e ? (dj * HR + di) : tap;
-        }
-    const double *w = halo + idx0;
-    if (c_eq == 1) return w[tap];
-    double vmin = INFINITY, vmax = -INFINITY;     // several taps under the median's key
-    for (int dj = 0; dj < D; ++dj)
-        for (int di = 0; di < D; ++di)
-            if (q[dj * HR + di] == m) {
-                const double v = w[dj * HR + di];
-                vmin = v < vmin ? v : vmin;
-                vmax = v > vmax ? v : vmax;
-            }
-    if (vmin == vmax) return vmin;
-    if (stats) stats[1] += 1;
-    return window_median<4, ListT>(halo, halo0, HR, idx0, list, ls, D * D, stats);
 }
 
 }  // namespace icnv

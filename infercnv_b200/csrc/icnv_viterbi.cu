@@ -66,13 +66,6 @@ struct VitParams {
     double tau;                // decision-margin threshold below which a sequence is re-run exactly
     const double *table;       // device copy of icnv_emis_table
     int means_monotone;        // state means sorted (either direction): the furthest state from any x is an end state
-    const float4 *table32;     // device copy of icnv_emis_table32 (single-precision first pass)
-    // sequences the single-precision pass could not certify, grouped by (sorted) chromosome so that a warp of the FP64 pass
-    // still works on 32 sequences of one length: seq_cells[ks * C + i], i < seq_counts[ks]
-    int32_t *seq_cells;
-    unsigned int *seq_counts;
-    int seq_mode;              // viterbi_fast_kernel: 1 = the items are tiles of those lists instead of tiles of all cells
-    int evict_first;           // L2 policies (ICNV_VIT_EVICT): 0 none, 1 input stream evict_first, 2 (default) ring stores evict_last, 3 = 2 + discard of read ring lines
     int2 *list_out;
     unsigned int *list_out_count;
     unsigned int list_cap;
@@ -339,37 +332,13 @@ __global__ void __launch_bounds__(128) viterbi_kernel(const VitParams p) {
 constexpr int FAST_MAX_N = 3600;   // longest sequence the error budget above certifies
 constexpr int TG = 8;        // genes per staged tile
 constexpr int TS = TG + 1;   // padded row stride in doubles (bank-conflict-free column reads)
-constexpr int FAST_WARPS = 16;   // default warps per CTA (one CTA per SM: the replicated table below is shared by all of them);
-                                 // 20 / 24 are compiled as occupancy variants (ICNV_VFAST_WARPS): 96 / 80 registers per thread,
-                                 // the gene loop stays spill-free, ~19 values are re-loaded from local memory per 8-gene tile
+constexpr int FAST_WARPS = 16;   // warps per CTA (one CTA per SM: the replicated table below is shared by all of them)
 constexpr int TAB_REP = 8;       // table replicas: lane l reads replica l & 7, so a 16-byte lookup never bank-conflicts
 
-// L2 policies around the backpointer rings (16 warps x 132 SMs x the longest chromosome x 128 bytes: more than the 50 MB L2
-// of an H100 holds beside the input stream).  ICNV_VIT_EVICT selects one; DESIGN.md section 3 K3 has the measured choice.
-__device__ __forceinline__ unsigned long long l2_evict_first_policy(int evict_first) {
-    unsigned long long pol;
-    if (evict_first) asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    else asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-// backpointer store with an L2 policy (ICNV_VIT_EVICT=2: the ring is kept with evict_last, the input stream is read normally)
-__device__ __forceinline__ unsigned long long l2_evict_last_policy() {
-    unsigned long long pol;
-    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
-// drop one 128-byte line of the ring from L2 WITHOUT writing it back: the trace-back has read it, the next sequence overwrites it
-__device__ __forceinline__ void l2_discard_line(const void *line) {
-    asm volatile("discard.global.L2 [%0], 128;" ::"l"(line) : "memory");
-}
-__device__ __forceinline__ void bp_store(uint16_t *ptr, uint16_t v, unsigned long long pol, bool hinted) {
-    if (hinted) asm volatile("st.global.L2::cache_hint.u16 [%0], %1, %2;" ::"l"(ptr), "h"(v), "l"(pol) : "memory");
-    else *ptr = v;
-}
-__device__ __forceinline__ void cp_async8(void *smem_dst, const void *gsrc, bool valid, unsigned long long pol) {
+__device__ __forceinline__ void cp_async8(void *smem_dst, const void *gsrc, bool valid) {
     unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     int sz = valid ? 8 : 0;  // src-size 0: zero-fill, nothing is read
-    asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 8, %2, %3;\n" ::"r"(d), "l"(gsrc), "r"(sz), "l"(pol) : "memory");
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(d), "l"(gsrc), "r"(sz) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N>
@@ -449,8 +418,6 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
     uint16_t *__restrict__ bp = reinterpret_cast<uint16_t *>(p.bp + warp_global * (int64_t)p.max_len * 32);
     const double cmove = p.cmove;   // read from the parameter bank where it is used: no register held for it
     const double MAGIC = 6755399441055744.0;  // 1.5 * 2^52: (v + MAGIC) - MAGIC == rint(v), low word == (int)rint(v)
-    const unsigned long long pol = l2_evict_first_policy(p.evict_first == 1);
-    const unsigned long long pol_ring = l2_evict_last_policy();
     // a state is "near the best" when its e = score - (best - cmove) reaches cmove - tau (> 0: the launcher refuses the fast
     // path unless cmove > 8 tau).  Compared by high words: e >= cmove - tau implies hi(e) >= lim_hi, so the count can only
     // come out too large - i.e. the check rejects a little more than the exact one would (a gap below tau + one unit of the
@@ -458,45 +425,19 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
     const int lim_hi = p.near_hi;   // __double2hiint(cmove - tau), from the launcher (a parameter-bank operand)
     int err = 0;
 
-    const bool seq_compact = p.seq_mode && p.K <= 32;
     for (;;) {
         unsigned long long item = 0;
         if (lane == 0) item = atomicAdd(p.counter, 1ull);
-        // second pass with at most 32 chromosomes: lane l holds the number of 32-sequence tiles of chromosomes 0 .. l (a warp
-        // scan of the list lengths), an item number below the total names (chromosome, tile) directly - no empty items are
-        // drawn.  Formed per item: held across the gene loop, the two words would be spilled
-        unsigned seq_pre = 0, seq_total = 0;   // at most C + 32 tiles
-        if (seq_compact) {
-            unsigned t = lane < p.K ? (p.seq_counts[lane] + 31) / 32 : 0;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const unsigned u = __shfl_up_sync(0xffffffffu, t, d);
-                if (lane >= d) t += u;
-            }
-            seq_pre = t;
-            seq_total = __shfl_sync(0xffffffffu, t, 31);
-        }
         item = __shfl_sync(0xffffffffu, item, 0);
-        if ((int64_t)item >= (seq_compact ? seq_total : p.n_items)) break;
-        int ks = (int)(item / (unsigned long long)p.n_tiles);
-        int64_t tile = (int64_t)(item % (unsigned long long)p.n_tiles);
-        if (seq_compact) {
-            ks = __popc(__ballot_sync(0xffffffffu, seq_pre <= item));
-            const unsigned before = __shfl_sync(0xffffffffu, seq_pre, (ks + 31) & 31);   // lane ks - 1 (unused for ks = 0)
-            tile = (int64_t)item - (ks > 0 ? before : 0);
-        }
+        if ((int64_t)item >= p.n_items) break;
+        const int ks = (int)(item / (unsigned long long)p.n_tiles);
+        const int64_t tile = (int64_t)(item % (unsigned long long)p.n_tiles);
         const int cs = p.item_chr_start[ks];
         const int n = p.item_chr_len[ks];
         const int64_t c0 = tile * 32;
-        int64_t c = c0 + lane;
-        bool active = c < p.C;
-        if (p.seq_mode) {   // second pass: lane = entry c0 + lane of this chromosome's list of uncertified sequences
-            const int64_t cnt = (int64_t)p.seq_counts[ks];
-            if (c0 >= cnt) continue;
-            active = c0 + lane < cnt;
-            c = (int64_t)p.seq_cells[(int64_t)ks * p.C + (active ? c0 + lane : c0)];
-        }
-        const int64_t cc = active ? c : (p.seq_mode ? c : p.C - 1);
+        const int64_t c = c0 + lane;
+        const bool active = c < p.C;
+        const int64_t cc = active ? c : (p.C - 1);
         uint8_t *__restrict__ scol = p.states + p.G * cc;
         if (n < 2) {
             if (active && n == 1) scol[cs] = 3;
@@ -525,9 +466,8 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                 const int row = q * 4 + (lane >> 3);
                 int64_t cell = c0 + row;
                 if (cell >= p.C) cell = p.C - 1;
-                if (p.seq_mode) cell = __shfl_sync(0xffffffffu, (int)cc, row);   // the cell of lane `row`
                 const double *src = p.X + p.G * cell + (ok ? gene : 0);
-                cp_async8(dst + row * TS + col, src, ok, pol);
+                cp_async8(dst + row * TS + col, src, ok);
             }
         };
 
@@ -648,7 +588,7 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                     nu[k] = (stay ? nu[k] : T) + le[k];
                     moved = __funnelshift_l((uint32_t)he, moved, 1);
                 }
-                bp_store(bp + (int64_t)i * 32 + lane, (uint16_t)(moved | ((uint32_t)i1 << 8)), pol_ring, p.evict_first >= 2);
+                bp[(int64_t)i * 32 + lane] = (uint16_t)(moved | ((uint32_t)i1 << 8));
             }
             __syncwarp();
         }
@@ -684,7 +624,6 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
         // ---- traceback in aligned blocks of 8 genes: the 8 backpointer words are loaded together
         //      (independent addresses), states leave as one 8-byte word when the layout allows it -----
         const bool wide = ((p.G & 7) == 0);  // then (G*c + g) is 8-aligned whenever g is
-        int ring_front = (n + 1) >> 1;       // ICNV_VIT_EVICT=3: 128-byte lines (two gene rows) of the ring at and above this one are dead
         for (int gb = (g_hi - 1) & ~7; gb + 8 > g_lo; gb -= 8) {
             uint32_t w[8];
 #pragma unroll
@@ -700,254 +639,11 @@ __global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast_kernel(const VitP
                     pack |= (unsigned long long)(y + 1) << (8 * q);
                     if (g > g_lo) y = ((w[q] >> y) & 1u) ? (int)(w[q] >> 8) : y;
                 }
-            }
-            if (p.evict_first == 3) {   // every lane has consumed its words of the rows >= gb - g_lo: those lines are dead
-                __syncwarp();
-                const int first = (max(gb - g_lo, 0) + 1) >> 1;   // first line that lies wholly in rows >= gb - g_lo
-                if (first + lane < ring_front) l2_discard_line(bp + (int64_t)(first + lane) * 64);
-                ring_front = min(ring_front, first);
             }
             if (active) {
                 if (wide && gb >= g_lo && gb + 8 <= g_hi) {
                     *reinterpret_cast<unsigned long long *>(scol + gb) = pack;
                 } else {  // ragged first / last block of the chromosome, or unaligned layout
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const int g = gb + q;
-                        if (g >= g_lo && g < g_hi) scol[g] = (uint8_t)(pack >> (8 * q));
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    }
-    if (err && p.err_flag) atomicOr(p.err_flag, err);
-}
-
-// =================================================================================================
-// single-precision first pass of the certified fast path (hmm mode 2, an option: measured slower than the FP64 pass alone)
-// =================================================================================================
-//
-// The FP64 fast kernel above spends a third of its issue slots on half-rate FP64 instructions.  Almost every sequence
-// can be decided in SINGLE precision if the certificate is made sharper: what has to be certain is not every arg-max of
-// the recursion but only the ones ON THE PATH the trace-back follows.  So every state carries, next to its score, the
-// smallest winner / runner-up gap met along the best path into it (mg[k], inherited from the state the path comes from);
-// the sequence is certified when the final state's margin and the final arg-max gap exceed tau_n = eps32 * n.
-//
-// Error budget (eps32): the scores are kept in a moving frame - every gene subtracts (best previous score + 1/2) from all
-// states, a COMMON shift that no difference sees - so they stay in [-20.1, 0) where half an ulp is <= 9.6e-7.  A path
-// collects per gene: the emission (table + float evaluation, ICNV_EMIS32_ERR = 5.7e-7 against the double table, which is
-// itself within 5e-13 of 50-digit arithmetic), two roundings (the shift, the emission add) and, on a move, the rounded
-// constant b - a - 1/2: <= 3.5e-6 per gene.  Two paths differ by at most twice that; eps32 = 1.6e-5 per gene leaves a factor
-// of two.  The three low mantissa bits that carry the state index through the arg-max (first-index rule: scores are
-// negative, so among equal scores the lowest index is the largest key) only perturb the common shift and the best-vs-second
-// gap by < 8 ulp = 4e-6, far below tau_n.
-// Sequences that are not certified - a real change of state decided by less than tau_n (about 1 % of the transitions), an
-// input beyond the table, a non-finite value - go to the list and are recomputed by the reference-order kernel, exactly
-// like the rejects of the FP64 pass.
-#include "icnv_emission_table32.inc"
-
-constexpr float VF32_EPS = 1.6e-5f;   // certified margin per gene of the sequence (see above)
-constexpr float VF32_BIG = 1.0e30f;
-
-// float4 entry `idx` of the lane's table replica: one multiply-add for the address
-__device__ __forceinline__ float4 table_entry32(const float4 *tab_lane, int idx) {
-    const unsigned base = (unsigned)__cvta_generic_to_shared(tab_lane);   // loop-invariant
-    unsigned addr;
-    float4 c;
-    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(addr) : "r"((unsigned)idx), "n"(TAB_REP * 16), "r"(base));
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(c.x), "=f"(c.y), "=f"(c.z), "=f"(c.w) : "r"(addr));
-    return c;
-}
-
-template <int M, int NWARPS>
-__global__ void __launch_bounds__(NWARPS * 32, 1) viterbi_fast32_kernel(const VitParams p) {
-    extern __shared__ __align__(16) double sm[];
-    constexpr int NTAB = (ICNV_EMIS_N + 1) * TAB_REP;
-    float4 *tab = reinterpret_cast<float4 *>(sm);   // [interval][replica]: lane l reads replica l & 7 (see the FP64 kernel)
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    double *tiles = reinterpret_cast<double *>(tab + NTAB) + warp * (2 * 32 * TS);   // two staged x tiles per warp
-    for (int e = threadIdx.x; e < ICNV_EMIS_N * TAB_REP; e += blockDim.x) tab[e] = p.table32[e / TAB_REP];
-    __syncthreads();
-    const float4 *tab_lane = tab + (lane & (TAB_REP - 1));
-
-    const int64_t warp_global = (int64_t)blockIdx.x * NWARPS + warp;
-    uint16_t *__restrict__ bp = reinterpret_cast<uint16_t *>(p.bp + warp_global * (int64_t)p.max_len * 32);
-    const float T1p = (float)(p.b_off - p.a_diag - 0.5);   // "come from the best state" in the frame where that state's stay is -1/2
-    const float MAGIC = 12582912.0f;                        // 1.5 * 2^23: (v + MAGIC) - MAGIC == rintf(v), low bits == (int)rintf(v)
-    const unsigned long long pol = l2_evict_first_policy(p.evict_first == 1);
-    const unsigned long long pol_ring = l2_evict_last_policy();
-    int err = 0;
-
-    for (;;) {
-        unsigned long long item = 0;
-        if (lane == 0) item = atomicAdd(p.counter, 1ull);
-        item = __shfl_sync(0xffffffffu, item, 0);
-        if ((int64_t)item >= p.n_items) break;
-        const int ks = (int)(item / (unsigned long long)p.n_tiles);
-        const int64_t tile = (int64_t)(item % (unsigned long long)p.n_tiles);
-        const int cs = p.item_chr_start[ks];
-        const int n = p.item_chr_len[ks];
-        const int64_t c0 = tile * 32;
-        const int64_t c = c0 + lane;
-        const bool active = c < p.C;
-        const int64_t cc = active ? c : (p.C - 1);
-        uint8_t *__restrict__ scol = p.states + p.G * cc;
-        if (n < 2) {
-            if (active && n == 1) scol[cs] = 3;
-            continue;
-        }
-        const double sd = p.sd_col ? p.sd_col[cc] : p.sd;
-        const double scale = (double)ICNV_EMIS_INVW / sd;   // zs = 16 * |x - mean| / sd, formed in double: x - mean cancels
-        double nms[MAXM];
-#pragma unroll
-        for (int k = 0; k < M; ++k) nms[k] = -p.mean[k] * scale;
-        const int g_lo = cs, g_hi = cs + n;
-        const int b_first = g_lo / TG, b_last = (g_hi - 1) / TG;
-
-        auto issue_tile = [&](int blk, int buf) {
-            double *dst = tiles + buf * (32 * TS);
-            const int col = lane & 7;
-            const int64_t gene = (int64_t)blk * TG + col;
-            const bool ok = gene < p.G;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const int row = q * 4 + (lane >> 3);
-                int64_t cell = c0 + row;
-                if (cell >= p.C) cell = p.C - 1;
-                const double *src = p.X + p.G * cell + (ok ? gene : 0);
-                cp_async8(dst + row * TS + col, src, ok, pol);
-            }
-        };
-
-        float nu[MAXM], mg[MAXM];
-        bool dead = false;   // something the single-precision pass does not handle: the sequence goes to the exact kernel
-        issue_tile(b_first, 0);
-        cp_async_commit();
-        for (int blk = b_first; blk <= b_last; ++blk) {
-            const int buf = (blk - b_first) & 1;
-            if (blk < b_last) {
-                issue_tile(blk + 1, buf ^ 1);
-                cp_async_commit();
-                cp_async_wait<1>();
-            } else {
-                cp_async_wait<0>();
-            }
-            __syncwarp();
-            const double *row = tiles + buf * (32 * TS) + lane * TS;
-            const int j0 = max(0, g_lo - blk * TG), j1 = min(TG, g_hi - blk * TG);
-#pragma unroll 1
-            for (int j = j0; j < j1; ++j) {
-                const int i = blk * TG + j - g_lo;
-                const double x = row[j];
-                // ---- emissions: g(z_k) from the single-precision table ----------------------------------
-                double zs[MAXM];
-                float le[MAXM];
-#pragma unroll
-                for (int k = 0; k < M; ++k) zs[k] = fabs(fma(x, scale, nms[k]));
-                const double LIM = (double)(ICNV_EMIS_N - 1);
-                bool in_table = (zs[0] < LIM) && (zs[M - 1] < LIM);   // also false for a non-finite x
-                if (!p.means_monotone) {
-#pragma unroll
-                    for (int k = 1; k < M - 1; ++k) in_table = in_table && (zs[k] < LIM);
-                }
-                if (in_table) {
-#pragma unroll
-                    for (int k = 0; k < M; ++k) {
-                        const float zf = (float)zs[k];
-                        const float m = zf + MAGIC;
-                        const float u = zf - (m - MAGIC);
-                        const float4 cf = table_entry32(tab_lane, __float_as_int(m) & 0x3ff);
-                        le[k] = fmaf(u, fmaf(u, cf.z, cf.y), cf.x);
-                    }
-                } else {   // beyond the table or non-finite: the exact kernel decides (and raises the error flags)
-                    if (!is_finite_d(x)) err |= 1;
-                    dead = true;
-#pragma unroll
-                    for (int k = 0; k < M; ++k) le[k] = 0.0f;
-                }
-                if (i == 0) {
-#pragma unroll
-                    for (int k = 0; k < M; ++k) {
-                        nu[k] = ((float)p.logdelta[k] - 0.5f) + le[k];   // < 0: log delta <= 0, g <= 0.367
-                        mg[k] = VF32_BIG;
-                    }
-                    continue;
-                }
-                // ---- best and second best previous score.  All scores are negative, so the state index in the three low
-                //      mantissa bits makes the lowest index the largest among equal scores (which.max's first-index rule)
-                float k1 = __int_as_float((__float_as_int(nu[0]) & ~7) | 0), k2 = -VF32_BIG;
-#pragma unroll
-                for (int k = 1; k < M; ++k) {
-                    const float key = __int_as_float((__float_as_int(nu[k]) & ~7) | k);
-                    k2 = fmaxf(k2, fminf(k1, key));
-                    k1 = fmaxf(k1, key);
-                }
-                const int i1 = __float_as_int(k1) & 7;
-                const float g12 = k1 - k2;             // best minus second best (>= 0)
-                const float shift = -0.5f - k1;        // common to all states
-                float mg1 = mg[0];
-#pragma unroll
-                for (int k = 1; k < M; ++k) mg1 = (i1 == k) ? mg[k] : mg1;
-                const float cm = fminf(mg1, g12);      // a path that moves in: the best state's margin, and best vs second best
-                uint32_t moved = 0;
-#pragma unroll
-                for (int k = M - 1; k >= 0; --k) {
-                    const float d = nu[k] + shift;     // stay
-                    const float e = d - T1p;           // >= 0: stay wins (the runner-up is then the best state: gap e)
-                    const bool stay = e >= 0.0f;
-                    nu[k] = fmaxf(d, T1p) + le[k];
-                    mg[k] = fminf(stay ? mg[k] : cm, fabsf(e));
-                    moved = __funnelshift_l((uint32_t)__float_as_int(e), moved, 1);
-                }
-                bp_store(bp + (int64_t)i * 32 + lane, (uint16_t)(moved | ((uint32_t)i1 << 8)), pol_ring, p.evict_first >= 2);
-            }
-            __syncwarp();
-        }
-        // ---- termination ------------------------------------------------------------------------------
-        int y = 0;
-        float cert;
-        {
-            float best = nu[0], second = -VF32_BIG, mb = mg[0];
-#pragma unroll
-            for (int k = 1; k < M; ++k) {
-                if (nu[k] > best) {
-                    second = best;
-                    best = nu[k];
-                    mb = mg[k];
-                    y = k;
-                } else if (nu[k] > second) {
-                    second = nu[k];
-                }
-            }
-            cert = fminf(mb, best - second);
-        }
-        if (active && (dead || !(cert > VF32_EPS * (float)n))) {   // also catches NaN: to the FP64 pass
-            const unsigned pos = atomicAdd(p.seq_counts + ks, 1u);
-            p.seq_cells[(int64_t)ks * p.C + pos] = (int32_t)c;      // at most C entries per chromosome
-        }
-        // ---- traceback (as in the FP64 kernel) ----------------------------------------------------------
-        const bool wide = ((p.G & 7) == 0);
-        for (int gb = (g_hi - 1) & ~7; gb + 8 > g_lo; gb -= 8) {
-            uint32_t w[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const int i = gb + q - g_lo;
-                w[q] = (i >= 1 && i < n) ? (uint32_t)bp[(int64_t)i * 32 + lane] : 0u;
-            }
-            unsigned long long pack = 0;
-#pragma unroll
-            for (int q = 7; q >= 0; --q) {
-                const int g = gb + q;
-                if (g >= g_lo && g < g_hi) {
-                    pack |= (unsigned long long)(y + 1) << (8 * q);
-                    if (g > g_lo) y = ((w[q] >> y) & 1u) ? (int)(w[q] >> 8) : y;
-                }
-            }
-            if (active) {
-                if (wide && gb >= g_lo && gb + 8 <= g_hi) {
-                    *reinterpret_cast<unsigned long long *>(scol + gb) = pack;
-                } else {
 #pragma unroll
                     for (int q = 0; q < 8; ++q) {
                         const int g = gb + q;
@@ -1184,15 +880,6 @@ int icnv_dev_scatter_group_states(const uint8_t *gs, int64_t G, int64_t C, const
     return ICNV_OK;
 }
 
-// the certified FP64 kernel for m states, fw warps per CTA (16, 20 or 24) and a per-column or launch-wide sd
-static void (*fast_kernel_for(int m, int fw, bool sd_col))(const VitParams) {
-    if (sd_col)
-        return (m == 6) ? (fw == 24 ? viterbi_fast_kernel<6, 24, true> : (fw == 20 ? viterbi_fast_kernel<6, 20, true> : viterbi_fast_kernel<6, 16, true>))
-                        : (fw == 24 ? viterbi_fast_kernel<3, 24, true> : (fw == 20 ? viterbi_fast_kernel<3, 20, true> : viterbi_fast_kernel<3, 16, true>));
-    return (m == 6) ? (fw == 24 ? viterbi_fast_kernel<6, 24, false> : (fw == 20 ? viterbi_fast_kernel<6, 20, false> : viterbi_fast_kernel<6, 16, false>))
-                    : (fw == 24 ? viterbi_fast_kernel<3, 24, false> : (fw == 20 ? viterbi_fast_kernel<3, 20, false> : viterbi_fast_kernel<3, 16, false>));
-}
-
 int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len, int K,
                          int m, const double *Pi, const double *delta, const double *mean, const double *sd,
                          int sd_per_col, uint8_t *states_u8, double *margins, int *err_flag, void *stream) {
@@ -1258,20 +945,13 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
     p.margins = margins;
     p.err_flag = err_flag;
 
-    // counters: [0] work counter of the main launch, [1] work counter of the list launch, [2] list length, [3] work counter of
-    // the FP64 second pass; behind them K list lengths of the single-precision pass (one per sorted chromosome)
-    const size_t counter_bytes = 4 * sizeof(unsigned long long) + sizeof(unsigned int) * (size_t)K;
+    // counters: [0] work counter of the main launch, [1] work counter of the list launch, [2] list length
+    const size_t counter_bytes = 3 * sizeof(unsigned long long);
     unsigned long long *d_counter = (unsigned long long *)scratch(SLOT_MISC2, counter_bytes + 64);
     if (!d_counter) return ICNV_E_NOMEM;
     ICNV_CUDA(cudaMemsetAsync(d_counter, 0, counter_bytes, st));
     p.counter = d_counter;
     c.hmm_list_count = reinterpret_cast<unsigned int *>(d_counter + 2);
-    c.hmm_seq_counts = reinterpret_cast<unsigned int *>(d_counter + 4);
-    c.hmm_seq_k = 0;
-    p.evict_first = c.opt_vit_evict;
-    p.seq_mode = 0;
-    p.seq_cells = nullptr;
-    p.seq_counts = c.hmm_seq_counts;
 
     const bool want_margin = margins != nullptr;
     // the fast path needs .get_HMM's structure: one diagonal and one off-diagonal value
@@ -1283,11 +963,7 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
     // transition possible (log 0 would poison the margins): t <= 1/6 for i6, 1/3 for i3, and t > 0.  The certificate's
     // best-versus-others check reads the gap off e = stay - from_best, which needs log(diag / offdiag) well above tau.
     structured = structured && Pi[0] > Pi[1] && Pi[1] > 0.0 && std::log(Pi[0] / Pi[1]) > 1e-6;
-    const bool use_fast = (c.hmm_mode >= 1) && structured && !want_margin;
-    // mode 2 (default): single-precision first pass with per-path margins.  Its scores live in [b - a - 6.2, 0); the error
-    // budget assumes magnitudes below 32, i.e. log(diag / offdiag) <= 25 (t >= 1.4e-11) - beyond that the FP64 pass runs
-    bool use_fast32 = use_fast && c.hmm_mode == 2 && std::log(Pi[0] / Pi[1]) <= 25.0;
-    for (int k = 0; k < m; ++k) use_fast32 = use_fast32 && delta[k] >= 1e-30;   // log delta must fit the single-precision frame
+    const bool use_fast = (c.hmm_mode == 1) && structured && !want_margin;
 
     if (!use_fast) {
         int per_sm = 0;
@@ -1336,78 +1012,26 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
     p.list_cap = (unsigned int)std::min<size_t>(list_cap, 0xffffffffu);
 
     auto lkern = (m == 6) ? viterbi_list_kernel<6> : viterbi_list_kernel<3>;
-    if (use_fast32) {
-        float4 *d_table32 = (float4 *)scratch(SLOT_TABLE32, sizeof(icnv_emis_table32));
-        if (!d_table32) return ICNV_E_NOMEM;
-        if (!c.table32_uploaded) {
-            ICNV_CUDA(cudaMemcpyAsync(d_table32, icnv_emis_table32, sizeof(icnv_emis_table32), cudaMemcpyHostToDevice, st));
-            ICNV_CUDA(cudaStreamSynchronize(st));
-            c.table32_uploaded = true;
-        }
-        p.table32 = d_table32;
-        int fw = (c.opt_vfast_warps == 24 || c.opt_vfast_warps == 20) ? c.opt_vfast_warps : FAST_WARPS;
-        void (*fkern)(const VitParams) =
-            (m == 6) ? (fw == 24 ? viterbi_fast32_kernel<6, 24> : (fw == 20 ? viterbi_fast32_kernel<6, 20> : viterbi_fast32_kernel<6, 16>))
-                     : (fw == 24 ? viterbi_fast32_kernel<3, 24> : (fw == 20 ? viterbi_fast32_kernel<3, 20> : viterbi_fast32_kernel<3, 16>));
-        const size_t smem = sizeof(float4) * (ICNV_EMIS_N + 1) * TAB_REP + sizeof(double) * (size_t)fw * 2 * 32 * TS;
-        p.means_monotone = 1;
-        for (int k = 1; k + 1 < m; ++k)
-            if ((mean[k] - mean[k - 1]) * (mean[k + 1] - mean[k]) < 0.0) p.means_monotone = 0;
-        ICNV_CUDA(cudaFuncSetAttribute(fkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int64_t blocks = c.sm_count;
-        const int64_t need_blocks = (p.n_items + fw - 1) / fw;
-        if (blocks > need_blocks) blocks = need_blocks;
-        const int64_t list_blocks = c.sm_count;
-        const int64_t n_warps = std::max<int64_t>(std::max<int64_t>(blocks * fw, (int64_t)c.sm_count * FAST_WARPS), list_blocks * 4);
-        uint32_t *d_bp = (uint32_t *)scratch(SLOT_BP, sizeof(uint32_t) * (size_t)n_warps * (size_t)max_len * 32);
-        if (!d_bp) return ICNV_E_NOMEM;
-        p.bp = d_bp;
-        int32_t *d_seq = (int32_t *)scratch(SLOT_SEQ, sizeof(int32_t) * (size_t)K * (size_t)C);
-        if (!d_seq) return ICNV_E_NOMEM;
-        p.seq_cells = d_seq;
-        c.hmm_seq_k = K;
-        fkern<<<(unsigned)blocks, fw * 32, smem, st>>>(p);
-        ICNV_CHECK_LAUNCH("viterbi_fast32_kernel");
-        // second pass: the sequences the single-precision margins could not certify, 32 of one chromosome per warp, in the FP64
-        // arithmetic with its own (all-decisions) certificate; what that rejects goes on to the reference-order kernel
-        void (*fkern64)(const VitParams) = fast_kernel_for(m, FAST_WARPS, sd_per_col != 0);
-        const size_t smem64 = sizeof(double) * (4 * (ICNV_EMIS_N + 1) * TAB_REP + (size_t)FAST_WARPS * 2 * 32 * TS);
-        ICNV_CUDA(cudaFuncSetAttribute(fkern64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem64));
-        p.seq_mode = 1;
-        p.counter = d_counter + 3;
-        const int64_t blocks64 = std::min<int64_t>(c.sm_count, (n_warps + FAST_WARPS - 1) / FAST_WARPS);
-        fkern64<<<(unsigned)blocks64, FAST_WARPS * 32, smem64, st>>>(p);
-        ICNV_CHECK_LAUNCH("viterbi_fast_kernel (second pass)");
-        p.seq_mode = 0;
-        p.list = d_list;
-        p.list_count = c.hmm_list_count;
-        p.counter = d_counter + 1;
-        lkern<<<(unsigned)list_blocks, LIST_NT, 0, st>>>(p);
-        ICNV_CHECK_LAUNCH("viterbi_list_kernel");
-        return ICNV_OK;
-    }
-    // warps per CTA of the fast kernel: 16 (128 registers per thread) unless ICNV_VFAST_WARPS picks an occupancy variant
-    int fw = FAST_WARPS;
-    if (c.opt_vfast_warps) fw = c.opt_vfast_warps;   // read once in icnv_init
-    if (fw != 16 && fw != 20 && fw != 24) fw = FAST_WARPS;
-    void (*fkern)(const VitParams) = fast_kernel_for(m, fw, sd_per_col != 0);
-    const size_t smem = sizeof(double) * (4 * (ICNV_EMIS_N + 1) * TAB_REP + (size_t)fw * 2 * 32 * TS);
+    void (*fkern)(const VitParams) = sd_per_col
+        ? ((m == 6) ? viterbi_fast_kernel<6, FAST_WARPS, true> : viterbi_fast_kernel<3, FAST_WARPS, true>)
+        : ((m == 6) ? viterbi_fast_kernel<6, FAST_WARPS, false> : viterbi_fast_kernel<3, FAST_WARPS, false>);
+    const size_t smem = sizeof(double) * (4 * (ICNV_EMIS_N + 1) * TAB_REP + (size_t)FAST_WARPS * 2 * 32 * TS);
     p.means_monotone = 1;
     for (int k = 1; k + 1 < m; ++k)
         if ((mean[k] - mean[k - 1]) * (mean[k + 1] - mean[k]) < 0.0) p.means_monotone = 0;
     ICNV_CUDA(cudaFuncSetAttribute(fkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    ICNV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fkern, fw * 32, smem));
+    ICNV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fkern, FAST_WARPS * 32, smem));
     if (per_sm < 1) per_sm = 1;
     int64_t blocks = (int64_t)c.sm_count * per_sm;
-    int64_t need_blocks = (p.n_items + fw - 1) / fw;
+    int64_t need_blocks = (p.n_items + FAST_WARPS - 1) / FAST_WARPS;
     if (blocks > need_blocks) blocks = need_blocks;
     const int64_t list_blocks = c.sm_count;  // 4 warps each; the list is short
-    const int64_t n_warps = std::max<int64_t>(blocks * fw, list_blocks * 4);
+    const int64_t n_warps = std::max<int64_t>(blocks * FAST_WARPS, list_blocks * 4);
     uint32_t *d_bp = (uint32_t *)scratch(SLOT_BP, sizeof(uint32_t) * (size_t)n_warps * (size_t)max_len * 32);
     if (!d_bp) return ICNV_E_NOMEM;
     p.bp = d_bp;
-    fkern<<<(unsigned)blocks, fw * 32, smem, st>>>(p);
+    fkern<<<(unsigned)blocks, FAST_WARPS * 32, smem, st>>>(p);
     ICNV_CHECK_LAUNCH("viterbi_fast_kernel");
     // exact re-run of whatever the certificate rejected (list length is read on the device)
     p.list = d_list;
@@ -1419,23 +1043,14 @@ int icnv_dev_viterbi_f64(const double *X, int64_t G, int64_t C, const int32_t *c
 }
 
 int icnv_set_hmm_mode(int mode) {
-    if (mode < 0 || mode > 2)
-        return set_error(ICNV_E_BAD_ARG, "hmm mode must be 0 (reference-order), 1 (certified FP64 pass) or 2 (certified FP32 pass, default)");
+    if (mode != 0 && mode != 1)
+        return set_error(ICNV_E_BAD_ARG, "hmm mode must be 0 (reference-order arithmetic) or 1 (certified FP64 pass, default), got %d", mode);
     ctx().hmm_mode = mode;
     return ICNV_OK;
 }
 
-/* sequences the single-precision pass of the last Viterbi call handed to the FP64 pass (0 in the other modes) */
-int64_t icnv_hmm_second_pass_count(void) {
-    Ctx &c = ctx();
-    if (!c.ready || !c.hmm_seq_counts || c.hmm_seq_k <= 0) return 0;
-    std::vector<unsigned int> h((size_t)c.hmm_seq_k);
-    cudaDeviceSynchronize();
-    if (cudaMemcpy(h.data(), c.hmm_seq_counts, sizeof(unsigned int) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    int64_t n = 0;
-    for (unsigned int v : h) n += v;
-    return n;
-}
+/* always 0: no HMM mode hands sequences to a second pass (kept for callers of the C ABI) */
+int64_t icnv_hmm_second_pass_count(void) { return 0; }
 
 int64_t icnv_hmm_rerun_count(void) {
     Ctx &c = ctx();

@@ -43,14 +43,9 @@ PTX_STANDINS = {
     "mbar_wait": "{ while (((*reinterpret_cast<volatile unsigned long long *>(bar)) & 1ull) == parity) emu::spin_yield(); }",
     "fence_proxy_async": "{ }",
     "cp_async8": "{ if (valid) memcpy(smem_dst, gsrc, 8); else memset(smem_dst, 0, 8); }",
-    "l2_evict_first_policy": "{ return 0ull; }",
-    "l2_evict_last_policy": "{ return 0ull; }",
-    "l2_discard_line": "{ (void)line; }",
-    "bp_store": "{ (void)pol; (void)hinted; *ptr = v; }",
     "cp_async_commit": "{ }",
     "cp_async_wait": "{ }",
     "count_if_ge": "{ acc += (v >= lim) ? 1 : 0; }",
-    "table_entry32": "{ return tab_lane[(size_t)idx * TAB_REP]; }",
     "table_entry": "{ const double2 *t = tab_lane + (size_t)idx * TAB_REP; c01 = t[0]; c2f = t[(ICNV_EMIS_N + 1) * TAB_REP]; }",
 }
 DYN_SMEM = re.compile(r"extern\s+__shared__\s+(?:__align__\(\d+\)\s+)?(?P<type>[\w ]+?)\s+(?P<name>\w+)\[\];")
@@ -60,7 +55,7 @@ LAUNCH = re.compile(r"(?P<name>[A-Za-z_]\w*(?:<[^<>();]*>)?)\s*<<<(?P<cfg>.*?)>>
 
 def replace_body(text: str, fn: str, body: str) -> str:
     """Swap the brace-delimited body of the device function `fn` (the definition, not its calls)."""
-    m = re.search(r"(?:void|unsigned|long|float4)\s+" + fn + r"\s*\([^)]*\)\s*\{", text)
+    m = re.search(r"(?:void|unsigned|long)\s+" + fn + r"\s*\([^)]*\)\s*\{", text)
     if not m:
         return text
     depth, i = 1, m.end()

@@ -63,50 +63,6 @@ static int run(std::mt19937_64 &rng, int trials, unsigned *stats) {
 }
 
 
-// window_median_net81: full 9 x 9 windows through the key network; every kind of the generic test plus values closer together
-// than single precision resolves (distinct doubles under one key around the median: the routine must fall back and stay exact)
-static int run_net81(std::mt19937_64 &rng, int trials, unsigned *stats) {
-    constexpr int D = 9;
-    const int HR = D + 3, idx0 = 2;
-    std::vector<double> halo((size_t)HR * (D + 1)), halo0(halo.size());
-    std::vector<float> kf(halo.size());
-    std::vector<unsigned short> list((size_t)D * D * 4);
-    std::normal_distribution<double> nd(0.0, 1.0);
-    std::uniform_real_distribution<double> ud(0.0, 1.0);
-    int bad = 0;
-    for (int t = 0; t < trials; ++t) {
-        const int kind = t % 10;
-        std::vector<double> vals;
-        for (int dj = 0; dj < D; ++dj)
-            for (int di = 0; di < D; ++di) {
-                double v = 0.0;
-                switch (kind) {
-                    case 0: v = 1.0 + 0.1 * nd(rng); break;
-                    case 1: v = std::exp(nd(rng)); break;
-                    case 2: v = (ud(rng) < 0.6 ? 1.0 : 1.5) + 0.02 * nd(rng); break;
-                    case 3: v = (ud(rng) < 0.7) ? 1.000123 : 1.0 + 0.2 * nd(rng); break;
-                    case 4: v = (double)(1 + (int)(ud(rng) * 6.0)); break;
-                    case 5: v = 3.0; break;
-                    case 6: v = (ud(rng) < 0.5) ? (ud(rng) < 0.5 ? 0.0 : -0.0) : 0.01 * nd(rng); break;
-                    case 7: v = 1.0 + 1e-9 * nd(rng); break;                 // all within a few float ulps of 1
-                    case 8: v = -2.5 + 1e-12 * (double)(int)(ud(rng) * 5.0); break;   // five distinct doubles, one float key
-                    default: v = 1e300 * (1.0 + 0.3 * nd(rng)); break;      // keys overflow to +-inf
-                }
-                halo[idx0 + dj * HR + di] = v;
-                halo0[idx0 + dj * HR + di] = v;
-                kf[idx0 + dj * HR + di] = (float)v;
-                vals.push_back(v);
-            }
-        const double want = ref_median(vals);
-        const double got = icnv::window_median_net81(halo.data(), halo0.data(), kf.data(), HR, idx0, list.data(), 3, stats);
-        if (!(got == want)) {
-            if (bad < 5) std::printf("net81 trial %d kind %d: got %.17g want %.17g\n", t, kind, got, want);
-            ++bad;
-        }
-    }
-    return bad;
-}
-
 int main(int argc, char **argv) {
     const int trials = argc > 1 ? std::atoi(argv[1]) : 20000;
     // sorting network: 0-1 principle
@@ -129,10 +85,5 @@ int main(int argc, char **argv) {
     bad += run<5>(rng, trials, stats);
     std::printf("windows %d, mismatches %d, list rounds per window %.2f, second build passes per window %.3f\n", 4 * trials, bad,
                 stats[0] / (4.0 * trials), stats[1] / (4.0 * trials));
-    unsigned nstats[2] = {0, 0};
-    const int nbad = run_net81(rng, trials, nstats);
-    std::printf("key network (9 x 9): windows %d, mismatches %d, fell back to the general routine %.3f per window\n", trials, nbad,
-                nstats[1] / (double)trials);
-    bad += nbad;
     return bad ? 1 : 0;
 }

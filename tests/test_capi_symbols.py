@@ -50,6 +50,15 @@ def test_cell_kernel_query_is_declared_and_bound():
     assert hasattr(_lib.load(), "icnv_debug_cell_kernel")
 
 
+def test_hmm_mode_other_than_0_or_1_is_refused():
+    """icnv_set_hmm_mode takes 0 (reference-order arithmetic) and 1 (certified FP64 pass); any other mode, 2 included, is
+    ICNV_E_BAD_ARG.  The mode is host state: no device is needed."""
+    from infercnv_b200 import _lib
+    lib = _lib.load()
+    assert lib.icnv_set_hmm_mode(2) == -3 and b"hmm mode" in lib.icnv_last_error()
+    assert lib.icnv_set_hmm_mode(1) == 0
+
+
 def test_product_never_imports_the_oracle():
     pkg = os.path.join(ROOT, "infercnv_b200")
     for dirpath, _, files in os.walk(pkg):

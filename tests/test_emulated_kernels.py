@@ -34,14 +34,11 @@ def test_gpu_parity_tests_pass_under_the_host_emulation(order):
 
 
 @pytest.mark.skipif(shutil.which("g++") is None and not os.path.exists("/usr/bin/g++"), reason="no host compiler")
-@pytest.mark.parametrize("env", [{"ICNV_VFAST_WARPS": "24"}, {"ICNV_VFAST_WARPS": "20"}, {"ICNV_HMM_MODE": "2"},
-                                 {"ICNV_CELL_PADQ": "0"}, {"ICNV_CELL_KERNEL": "4"}, {"ICNV_MF_KERNEL": "2"}, {"ICNV_MF_KERNEL": "5"}], ids=lambda e: "-".join(f"{k}={v}" for k, v in e.items()))
+@pytest.mark.parametrize("env", [{"ICNV_CELL_PADQ": "0"}, {"ICNV_CELL_KERNEL": "4"}], ids=lambda e: "-".join(f"{k}={v}" for k, v in e.items()))
 def test_kernel_variants_behind_the_tuning_switches_under_the_host_emulation(env):
-    """The variants DESIGN.md section 8 lists (Viterbi occupancy variants, the single-precision first pass, the ping-pong layout of the two-buffer cell
-    pipeline and the single-buffer v4 kernel at gene counts where v3 is the default) through the parity tests of the path
-    they replace."""
-    pick = "viterbi and not scale and not oligo and not device_resident" if ("ICNV_VFAST_WARPS" in env or "ICNV_HMM_MODE" in env) else \
-        ("median_filter" if "ICNV_MF_KERNEL" in env else "golden or slow_paths or smooth_lengths or known or padded_q or benchmark_layout")
+    """The variants DESIGN.md section 8 lists (the ping-pong layout of the two-buffer cell pipeline and the single-buffer v4
+    kernel at gene counts where v3 is the default) through the parity tests of the path they replace."""
+    pick = "golden or slow_paths or smooth_lengths or known or padded_q or benchmark_layout"
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "host", "run_emulated.py"),
                         os.path.join(ROOT, "tests", "test_gpu_parity.py"), "-k", pick], capture_output=True, text=True, timeout=1500,
                        env=dict(os.environ, **env))

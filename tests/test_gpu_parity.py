@@ -292,7 +292,7 @@ def test_viterbi_cells_bit_identical(api, hmm_fixture, m):
     np.testing.assert_array_equal(got2, want)
 
 
-@pytest.mark.parametrize("mode", ["exact", "fast", "fast32"])
+@pytest.mark.parametrize("mode", ["exact", "fast"])
 def test_viterbi_modes_agree_with_oracle_at_scale(api, hmm_fixture, mode):
     """2e7 cell-genes of the bench's synthetic structure: the certified fast path and the
     reference-order path must both reproduce the oracle's states exactly."""
@@ -323,45 +323,6 @@ def test_viterbi_modes_agree_with_oracle_at_scale(api, hmm_fixture, mode):
         assert reruns == 0
     else:   # the certificates must certify: a pass that sends everything to the exact kernel would also "agree"
         assert reruns < 0.02 * C * len(lens)
-
-
-@pytest.mark.parametrize("m", [6, 3])
-def test_viterbi_single_precision_pass_on_segmental_changes(api, hmm_fixture, m):
-    """The FP32 first pass certifies a sequence from the margins ALONG ITS PATH only; real changes of state inside a
-    chromosome are where those margins get small.  Segments of random length, position and amplitude (some barely above
-    the decision boundary, some one gene long), a noisy and a nearly noise-free half: states identical to the oracle, and
-    the pass must still certify most sequences itself."""
-    rng = np.random.default_rng(1234 + m)
-    lens = np.array([400, 37, 250, 2, 120, 611])
-    cs = np.concatenate([[0], np.cumsum(lens)[:-1]])
-    G, C = int(lens.sum()), 160
-    if m == 6:
-        mean, sd = hmm_fixture["mean"], hmm_fixture["sd"]
-    else:
-        mean, sd = np.array([0.9, 1.0, 1.1]), np.array([0.05, 0.05, 0.05])
-    X = 1.0 + np.where(np.arange(C) < C // 2, 0.04, 0.002)[None, :] * rng.normal(size=(G, C))
-    levels = (mean - 1.0) if m == 3 else np.array([-0.55, -0.16, 0.02, 0.12, 0.24, 0.45])
-    for c in range(C):
-        for _ in range(rng.integers(0, 7)):
-            k = rng.integers(0, len(lens))
-            a = rng.integers(0, lens[k])
-            b = min(lens[k], a + rng.choice([1, 3, 10, 40, 150]))
-            X[cs[k] + a:cs[k] + b, c] += rng.choice(levels) * rng.uniform(0.3, 1.2)
-    X = np.asfortranarray(X)
-    Pi, delta = orc.hmm_params(m)
-    want = orc.viterbi_matrix(X, cs, lens, Pi, delta, mean, sd, nthreads=orc.max_threads())
-    assert len(np.unique(want)) >= 3                      # the data does change state
-    api.set_hmm_mode("fast32")
-    try:
-        got = api.viterbi(X, cs, lens, Pi, delta, mean, sd)
-        reruns = api.hmm_second_pass_count()
-    finally:
-        api.set_hmm_mode("fast")
-    n_seq = C * int(np.sum(lens >= 2))
-    changes = int(np.sum(want[1:] != want[:-1]))
-    print(f"\n[viterbi fp32 pass, m={m}] {changes} changes of state in {n_seq} sequences, {reruns} sequences handed to the FP64 pass")
-    np.testing.assert_array_equal(got, want)
-    assert reruns < 0.25 * n_seq
 
 
 @pytest.mark.parametrize("m,t", [(6, 0.18), (3, 0.4), (6, 0.0)])
@@ -426,18 +387,13 @@ def test_viterbi_rerun_of_long_sequences(api, hmm_fixture, m):
         mean, sd = np.array([0.5, 1.5, 3.0]), np.array([0.25] * 3)
         Pi, delta = orc.hmm_params(3, 1e-6)
     want = orc.viterbi_matrix(X, cs, lens, Pi, delta, mean, sd)
-    # the FP64 pass rejects every sequence that meets a tie anywhere (all three lengths reach the exact kernel); with the
-    # optional FP32 pass first only those whose tie lies on the path it returns get that far - same states either way
-    for mode in ("fast", "fast32"):
-        api.set_hmm_mode(mode)
-        try:
-            got = api.viterbi(X, cs, lens, Pi, delta, mean, sd)
-            reruns = api.hmm_rerun_count()
-        finally:
-            api.set_hmm_mode("fast")
-        np.testing.assert_array_equal(got, want)
-        assert reruns >= (3 * (C // 2) if mode == "fast" else 1)
-        print(f"\n[viterbi long re-runs, m={m}, {mode}] {reruns} of {3 * C} sequences re-run")
+    # the FP64 pass rejects every sequence that meets a tie anywhere: all three lengths reach the exact kernel
+    api.set_hmm_mode("fast")
+    got = api.viterbi(X, cs, lens, Pi, delta, mean, sd)
+    reruns = api.hmm_rerun_count()
+    np.testing.assert_array_equal(got, want)
+    assert reruns >= 3 * (C // 2)
+    print(f"\n[viterbi long re-runs, m={m}] {reruns} of {3 * C} sequences re-run")
 
 
 def test_viterbi_unstructured_transition_matrix_and_far_outliers(api, hmm_fixture):
@@ -569,37 +525,6 @@ def test_median_filter_vs_oracle(api, window_size):
     want = orc.median_filter(X, cs, lens, groups, window_size, nthreads=orc.max_threads())
     np.testing.assert_allclose(got, want, rtol=0, atol=1e-15)
     np.testing.assert_array_equal(got[:, 31], X[:, 31])
-
-
-def test_median_filter_key_network_variant_is_exact(api, monkeypatch):
-    """ICNV_MF_KERNEL=2: tiles whose windows are all full 9 x 9 ones (window_size 7) take the median from a comparator
-    network on single-precision keys (window_median_net81) and find its double in a second pass; edge tiles and ties the
-    keys cannot resolve go through the counting selection.  Same values as the default kernel and the oracle on smooth
-    values, a de-noised-like matrix (runs of one constant), state-like small integers and values closer together than single
-    precision resolves."""
-    rng = np.random.default_rng(9)
-    lens = [150, 41, 96, 7]
-    cs = np.concatenate([[0], np.cumsum(lens)[:-1]])
-    G, C = int(np.sum(lens)), 90
-    groups = [np.arange(0, 41), rng.permutation(np.arange(41, 70)), np.arange(70, 77), np.arange(77, 90)]
-    base = 1.0 + 0.1 * rng.normal(size=(G, C))
-    cases = {
-        "smooth": base,
-        "denoised": np.where(np.abs(base - 1.0) < 0.12, 1.000123, base),
-        "states": rng.integers(1, 7, size=(G, C)).astype(float),
-        "sub-float": 1.0 + 1e-10 * rng.integers(0, 50, size=(G, C)),
-    }
-    for name, X in cases.items():
-        X = np.asfortranarray(X)
-        monkeypatch.setenv("ICNV_MF_KERNEL", "2")
-        api.reinit()   # tuning switches are read once, at icnv_init
-        got = api.median_filter(X, cs, lens, groups, 7)
-        monkeypatch.delenv("ICNV_MF_KERNEL")
-        api.reinit()
-        ref = api.median_filter(X, cs, lens, groups, 7)
-        want = orc.median_filter(X, cs, lens, groups, 7, nthreads=orc.max_threads())
-        assert np.array_equal(got, ref), name
-        np.testing.assert_allclose(got, want, rtol=0, atol=1e-15, err_msg=name)
 
 
 def test_median_filter_shared_merge_kernel_edges_and_ties(api):

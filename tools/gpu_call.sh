@@ -6,7 +6,6 @@ timeout 900 python -m pytest tests -m gpu -x -q > gpurun_out/${tag}_pytest_gpu.l
 timeout 300 python tools/bench_extra.py > gpurun_out/${tag}_secondary_kernels.json 2> gpurun_out/${tag}_secondary.err; cut -c1-300 gpurun_out/${tag}_secondary_kernels.json; tail -3 gpurun_out/${tag}_secondary.err
 timeout 900 python bench.py --config c4 --no-cpu-baseline --no-e2e > gpurun_out/${tag}_bench_c4.json 2> gpurun_out/${tag}_bench_c4.err; tail -5 gpurun_out/${tag}_bench_c4.err
 timeout 600 python bench.py --config c2 --no-cpu-baseline --no-e2e > gpurun_out/${tag}_bench_c2.json 2> gpurun_out/${tag}_bench_c2.err; tail -5 gpurun_out/${tag}_bench_c2.err
-ICNV_MF_KERNEL=3 timeout 300 python tools/bench_extra.py 2>/dev/null | cut -c1-120
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:median_filter_merge -c 1 -f -o gpurun_out/${tag}_prof_mfmerge python tools/bench_extra.py > /dev/null 2>&1
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:viterbi_fast -s 3 -c 1 -f -o gpurun_out/${tag}_prof_vfast python bench.py --config c2 --no-cpu-baseline --no-e2e --steps 2 --warmup 1 > /dev/null 2>&1
 ls -la gpurun_out | tail -6
