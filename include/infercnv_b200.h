@@ -336,6 +336,36 @@ ICNV_API int icnv_cluster_groups_f64(const double *X, int64_t G, int64_t C, cons
  * ms of linkages} (device time summed over the waves); zeros before any call and after a call without a tree. */
 ICNV_API int icnv_debug_cluster_groups(double *out5);
 
+/* The shared-nearest-neighbour graph of .leiden_seurat_preprocess_routine (R/inferCNV_tumor_subclusters.R:699-723; Seurat 5's
+ * FindVariableFeatures(vst) -> ScaleData -> RunPCA(npcs) -> FindNeighbors(k.param), prune.SNN 1/15) on the group matrix
+ * X[, cells] (G x C, 0-based columns; cells NULL: all C):
+ *   1. mu_g and v_g (denominator n - 1) over the n cells;
+ *   2. the vst trend: direct local quadratic loess (span 0.3, tricube weights on the q = floor(0.3 m) nearest) of log10 v on
+ *      log10 mu over the m genes with v > 0; expected variance 10^fit, 0 for constant genes;
+ *   3. standardised variance sum_c min((x - mu) / s, sqrt(n))^2 / (n - 1), s = sqrt(expected variance) (0 where s = 0),
+ *      ranked decreasing, ties by lower index: the first min(n_features, G) genes are the variable features;
+ *   4. z = min((x - mu) / sqrt(v), 10) on the F non-constant variable features;
+ *   5. the top npcs eigenvectors V of Z Z^T (exact to ||C v - l v|| <= 1e-12 l_1), each signed so that its largest |entry| is
+ *      positive (ties: lower feature rank); embeddings E = Z^T V;
+ *   6. K12's exact k nearest cells in E (self included; distance, then position), and for every pair with
+ *      s = |N(i) & N(j)| >= 1, w = s / (k + (k - s)), dropped when w < 1/15.  Symmetric, diagonal kept (w = 1).
+ * The result stays in the library until the next call; *nnz is its number of graph entries and icnv_seurat_snn_fetch
+ * copies it out.  Bad sizes or an index out of range: ICNV_E_BAD_ARG; NaN / Inf in a listed column: ICNV_E_NONFINITE;
+ * k > 64, npcs > 16, n <= npcs, fewer than 3 genes in the loess window, F <= npcs, a non-constant gene with mean <= 0 (vst's
+ * log10 warns there), no convergence of the eigenpairs, or a group larger than the free device memory: ICNV_E_UNSUPPORTED. */
+ICNV_API int icnv_seurat_snn_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int n_features,
+                                 int npcs, int k, int64_t *nnz);
+/* Copies out the last SNN call's result; any pointer may be NULL.  row_ptr: n + 1; col (0-based, ascending per row) and w:
+ * nnz; features: min(n_features, G) 0-based gene indices in rank order; emb: npcs x n column-major (K12's layout);
+ * idx: n x k column-major, 0-based positions.  No result held: ICNV_E_BAD_ARG. */
+ICNV_API int icnv_seurat_snn_fetch(int64_t *row_ptr, int32_t *col, double *w, int32_t *features, double *emb, int32_t *idx);
+/* What the last SNN call did: out16 = {F, npcs used, eigen-iterations, largest ||C v_j - l_j v_j|| / l_1, l_npcs / l_npcs+1
+ * (inf when the block has no npcs+1-th value), standardised-variance gap between ranks n_features and n_features + 1 (inf
+ * when G <= n_features), local trend fits that were singular (where R's loess warns and the routine falls back), device ms
+ * of: statistics, trend, standardised variance + ranking, Gram matrix, eigenpairs, embeddings, kNN, SNN; hub rows that took
+ * the global-memory path}; zeros before any call. */
+ICNV_API int icnv_debug_seurat_snn(double *out16);
+
 /* mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52; run() step 21, R/inferCNV_ops.R:1509-1524) on the G x C matrix X:
  * get_DE_genes_basic's tests, BH and .mask_DE_genes' mask in one call.
  *   Groups (CSR, 0-based columns): n_ref >= 1 reference groups; n_sub >= 0 TESTED subclusters in R's loop order (observation
@@ -600,6 +630,10 @@ ICNV_API int icnv_dev_pairwise_dist_rows_f64(const double *x, int64_t n, int64_t
  * `stream`, which is then synchronised once to report non-finite input. */
 ICNV_API int icnv_dev_knn_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int k,
                               int32_t *idx, double *dist, void *stream);
+/* icnv_seurat_snn_f64 on device pointers: columns X + ldx * (d_cells ? d_cells[a] : a), a < n (a chromosome is X offset by
+ * its first gene, ldx unchanged).  Synchronises `stream`; the result stays in the library (icnv_seurat_snn_fetch). */
+ICNV_API int icnv_dev_seurat_snn_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n,
+                                     int n_features, int npcs, int k, int64_t *nnz, void *stream);
 /* icnv_hclust_f64 on a device "dist" vector: merge / height (device) as above, no order (icnv_hclust_order on the host
  * copy of merge).  Synchronises the stream once, after filling the matrix, to report non-finite input; the linkage itself
  * is enqueued on `stream`. */

@@ -68,6 +68,10 @@ SIGNATURES = {
     "icnv_cluster_groups_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, _P, _P, c_int, c_int, _P, _P, _P]),
     "icnv_dev_cluster_groups_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, c_i64, _P, _P, c_int, c_int, _P, _P, _P]),
     "icnv_debug_cluster_groups": (c_int, [_P]),
+    "icnv_seurat_snn_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, c_int, c_int, _P]),
+    "icnv_dev_seurat_snn_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, c_int, c_int, _P, _P]),
+    "icnv_seurat_snn_fetch": (c_int, [_P, _P, _P, _P, _P, _P]),
+    "icnv_debug_seurat_snn": (c_int, [_P]),
     "icnv_mask_non_de_f64": (c_int, [_P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double, c_int,
                                      ct.c_double, ct.c_double, ct.c_double, ct.c_uint64, _P, _P]),
     "icnv_dev_mask_non_de_f64": (c_int, [_P, c_i64, _P, c_i64, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,

@@ -7,6 +7,7 @@ library; nothing here computes on the CPU.
 from __future__ import annotations
 
 import ctypes as ct
+from collections import namedtuple
 
 import numpy as np
 
@@ -502,6 +503,51 @@ def cluster_groups_stats() -> dict:
     out = np.zeros(5, dtype=np.float64)
     _lib.check(_lib.load().icnv_debug_cluster_groups(_p(out)))
     return {"waves": int(out[0]), "widest": int(out[1]), "gather_ms": out[2], "dist_ms": out[3], "link_ms": out[4]}
+
+
+SeuratSNN = namedtuple("SeuratSNN", "indptr indices data features embeddings idx stats")
+SeuratSNN.__doc__ = """What seurat_snn returns: the graph as CSR (indptr int64 n + 1, indices int32, data float64; symmetric,
+columns ascending per row), the variable features (0-based gene indices in rank order), the embeddings (n x npcs), the kNN
+lists (n x k, 0-based positions) and the call's statistics (seurat_snn_stats)."""
+
+
+def _fetch_snn(nnz: int, n: int, nf: int, npcs: int, k: int) -> SeuratSNN:
+    indptr = np.empty(n + 1, dtype=np.int64)
+    indices = np.empty(max(nnz, 1), dtype=np.int32)
+    data = np.empty(max(nnz, 1), dtype=np.float64)
+    feats = np.empty(max(nf, 1), dtype=np.int32)
+    emb = np.empty((n, npcs), dtype=np.float64)       # row-major n x npcs = the library's npcs x n column-major
+    idx = np.empty((k, n), dtype=np.int32)             # column-major n x k
+    _lib.check(_lib.load().icnv_seurat_snn_fetch(_p(indptr), _p(indices), _p(data), _p(feats), _p(emb), _p(idx)))
+    return SeuratSNN(indptr, indices[:nnz], data[:nnz], feats[:nf], emb, np.ascontiguousarray(idx.T), seurat_snn_stats())
+
+
+def seurat_snn(X, k=20, cells=None, n_features=2000, npcs=10) -> SeuratSNN:
+    """The SNN graph .leiden_seurat_preprocess_routine builds with Seurat (vst variable features, ScaleData, RunPCA(npcs),
+    FindNeighbors(k.param = k)) on the columns `cells` (default all) of the genes x cells matrix X, computed exactly on the
+    device (icnv_seurat_snn_f64; see include/infercnv_b200.h for the contract)."""
+    X = _f64(X)
+    G, C = X.shape
+    idx = None if cells is None else _i32(cells)
+    n = C if idx is None else len(idx)
+    nnz = ct.c_int64(0)
+    _lib.check(_lib.load().icnv_seurat_snn_f64(_p(X), G, C, _p(idx), n, int(n_features), int(npcs), int(k),
+                                               ct.byref(nnz)))
+    return _fetch_snn(nnz.value, n, min(int(n_features), G), int(npcs), int(k))
+
+
+SNN_STAGES = ("stats", "trend", "stdvar", "gram", "eigen", "embed", "knn", "snn")
+
+
+def seurat_snn_stats() -> dict:
+    """What the last seurat_snn call did (icnv_debug_seurat_snn): F, npcs used, eigen-iterations, the largest relative
+    residual, the eigen-gap ratio, the standardised-variance gap at the n_features cut, singular trend fits, device ms per
+    stage and the hub rows that took the global-memory path."""
+    out = np.zeros(16, dtype=np.float64)
+    _lib.check(_lib.load().icnv_debug_seurat_snn(_p(out)))
+    return {"F": int(out[0]), "npcs": int(out[1]), "iterations": int(out[2]), "residual": out[3], "eig_ratio": out[4],
+            "sv_gap": out[5], "singular_fits": int(out[6]), "ms": dict(zip(SNN_STAGES, out[7:15].tolist())),
+            "hub_rows": int(out[15])}
 
 
 DE_TESTS = {"wilcoxon": 0, "t": 1}

@@ -2349,3 +2349,62 @@ int icnv_debug_cluster_groups(double *out5) {
 }
 
 }  // extern "C"
+
+// ---- Seurat's SNN graph, K18 (kernels and the device body in icnv_snn.cu) ---------------------------------------------------
+// Weak references, as for the linkage: a build without icnv_snn.cu reports them as unsupported.
+namespace icnv {
+int seurat_snn_check(int64_t G, int64_t n, int n_features, int npcs, int k, const char *who) __attribute__((weak));
+int seurat_snn_room(int64_t G, int64_t n, const char *who) __attribute__((weak));
+int seurat_snn_dev(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int n_features, int npcs,
+                   int k, int64_t *nnz, void *stream, const char *who) __attribute__((weak));
+int seurat_snn_fetch(int64_t *row_ptr, int32_t *col, double *w, int32_t *features, double *emb, int32_t *idx,
+                     cudaStream_t st, const char *who) __attribute__((weak));
+void seurat_snn_stats(double *out16) __attribute__((weak));
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_seurat_snn_f64(const double *X, int64_t G, int64_t C, const int32_t *cells, int64_t n, int n_features, int npcs,
+                        int k, int64_t *nnz) {
+    static const char *who = "icnv_seurat_snn_f64";
+    if (!icnv::seurat_snn_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no SNN kernels", who);
+    if (!cells) n = C;
+    if (!X || C < 1 || !nnz) return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    for (int64_t i = 0; cells && i < n; ++i)
+        if (cells[i] < 0 || cells[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index out of range", who);
+    int rc = icnv::seurat_snn_check(G, n, n_features, npcs, k, who);
+    if (rc) return rc;
+    ICNV_HOST_PROLOGUE();
+    if ((rc = icnv::seurat_snn_room(G, n, who))) return rc;
+    double *dX = nullptr;
+    int32_t *d_idx = nullptr;
+    if (cells) {
+        if ((rc = upload_listed_columns(X, G, cells, n, &dX, &d_idx, st))) return rc;
+    } else if ((rc = upload_matrix_ring(X, G * C, &dX, st))) {
+        return rc;
+    }
+    return icnv::seurat_snn_dev(dX, G, G, nullptr, n, n_features, npcs, k, nnz, st, who);
+}
+
+int icnv_dev_seurat_snn_f64(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int n_features,
+                            int npcs, int k, int64_t *nnz, void *stream) {
+    static const char *who = "icnv_dev_seurat_snn_f64";
+    if (!icnv::seurat_snn_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no SNN kernels", who);
+    return icnv::seurat_snn_dev(X, G, ldx, d_cells, n, n_features, npcs, k, nnz, stream, who);
+}
+
+int icnv_seurat_snn_fetch(int64_t *row_ptr, int32_t *col, double *w, int32_t *features, double *emb, int32_t *idx) {
+    static const char *who = "icnv_seurat_snn_fetch";
+    if (!icnv::seurat_snn_fetch) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no SNN kernels", who);
+    ICNV_HOST_PROLOGUE();
+    return icnv::seurat_snn_fetch(row_ptr, col, w, features, emb, idx, st, who);
+}
+
+int icnv_debug_seurat_snn(double *out16) {
+    if (!out16) return set_error(ICNV_E_BAD_ARG, "icnv_debug_seurat_snn: out16 is NULL");
+    for (int i = 0; i < 16; ++i) out16[i] = 0.0;
+    if (icnv::seurat_snn_stats) icnv::seurat_snn_stats(out16);
+    return ICNV_OK;
+}
+
+}  // extern "C"

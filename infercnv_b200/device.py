@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib, dist as shard
-from .api import _i32, groups_to_csr
+from .api import _fetch_snn, _i32, groups_to_csr
 
 _E_NONFINITE = -5   # ICNV_E_NONFINITE
 
@@ -412,6 +412,21 @@ class Engine:
         _lib.check(self.lib.icnv_dev_knn_f64(X.data_ptr(), G, max(X.stride(0), G), idx.data_ptr() if idx is not None else None,
                                              n, int(k), nn_idx.data_ptr(), nn_dist.data_ptr(), _stream_ptr()))
         return nn_idx.T, nn_dist.T
+
+    def seurat_snn(self, X, k=20, cells=None, n_features=2000, npcs=10):
+        """api.seurat_snn on the listed local cells (rows of X; default all) on the device: X is a (C, G) float64 tensor
+        with contiguous genes or a gene-range view of one (X[:, a:b], one chromosome - the per-chromosome PCA route).
+        Returns an api.SeuratSNN with host arrays (the graph goes to igraph on the host)."""
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        G = X.shape[1]
+        idx = None if cells is None else torch.as_tensor(np.asarray(cells, dtype=np.int32), device=self.tdev)
+        n = X.shape[0] if idx is None else int(idx.numel())
+        nnz = ct.c_int64(0)
+        _lib.check(self.lib.icnv_dev_seurat_snn_f64(X.data_ptr(), G, max(X.stride(0), G),
+                                                    idx.data_ptr() if idx is not None else None, n, int(n_features),
+                                                    int(npcs), int(k), ct.byref(nnz), _stream_ptr()))
+        return _fetch_snn(nnz.value, n, min(int(n_features), G), int(npcs), int(k))
 
     def hclust(self, D, n, method="ward.D2"):
         """hclust() on the device "dist" vector D of n observations (what pairwise_dist returns), fastcluster's methods

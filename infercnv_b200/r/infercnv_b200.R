@@ -596,6 +596,41 @@ b200_.parameterize_random_cluster_heights_smoothed_trees <- function(expr_matrix
     orig(expr_matrix, hclust_method, window_size, plot)
 }
 
+## .leiden_seurat_preprocess_routine (R/inferCNV_tumor_subclusters.R:699-723), the Leiden graph of step 15's default
+## leiden_method = "PCA" (per group, and per (chromosome, group) for leiden_method_per_chr = "PCA"): Seurat's
+## FindVariableFeatures(vst) -> ScaleData -> RunPCA(npcs = 10) -> FindNeighbors(k.param = k_nn) in one GPU call
+## (icnv_seurat_snn_f64), then igraph's graph_from_adjacency_matrix(mode = "min", weighted = TRUE) and cluster_leiden
+## exactly as the original calls them.  Deviations from the original:
+##  - irlba and annoy are approximate; the device computes what they approximate (exact eigenpairs, the exact kNN), so the
+##    graph can differ where annoy misses a neighbour or irlba's 1e-5 tolerance moves a near-tie;
+##  - vst's loess is the direct local fit; R's default surface = "interpolate" interpolates it on a kd-tree, so genes whose
+##    standardised variances lie within that interpolation error of the 2000th can be chosen differently
+##    (icnv_debug_seurat_snn reports the gap at the cut);
+##  - set.seed(42) is called where RunPCA(seed.use = 42) calls it, so the partition does not depend on the user's seed, as
+##    in the original; partitions are not claimed equal to R's draw for draw (irlba's draws are not replayed).
+## Falls back to the original for a matrix that is not double or holds NA, k_nn > 64, any library error (a non-constant
+## gene with mean <= 0 among them: vst's log10 warns there), or a singular local trend fit - where R's loess warns and the
+## original falls back to .leiden_simple_snn, which stays R's.
+b200_.leiden_seurat_preprocess_routine <- function(expr_data, k_nn, resolution_parameter, objective_function) {
+    orig <- .icnv_env$orig$.leiden_seurat_preprocess_routine
+    ok <- .icnv_enabled() && .icnv_ok(expr_data) && is.numeric(k_nn) && length(k_nn) == 1 && !is.na(k_nn) && k_nn >= 1 &&
+        k_nn <= 64 && k_nn <= ncol(expr_data)
+    if (ok) {
+        res <- .icnv_try(.Call("icnvR_seurat_snn", expr_data, as.integer(k_nn)), "the Seurat SNN graph")
+        if (!is.null(res) && res[[4]] == 0L) {
+            n <- ncol(expr_data)
+            snn <- Matrix::sparseMatrix(i = res[[2]], p = res[[1]], x = res[[3]], dims = c(n, n), index1 = FALSE,
+                                        dimnames = list(colnames(expr_data), colnames(expr_data)))
+            set.seed(42)
+            graph_obj <- igraph::graph_from_adjacency_matrix(snn, mode = "min", weighted = TRUE)
+            partition_obj <- igraph::cluster_leiden(graph_obj, resolution_parameter = resolution_parameter,
+                                                    objective_function = objective_function)
+            return(partition_obj$membership)
+        }
+    }
+    orig(expr_data, k_nn, resolution_parameter, objective_function)
+}
+
 ## mask_non_DE_genes_basic (R/inferCNV_mask_non_DE.R:28-52), run()'s step 21: every (subcluster, reference group) test,
 ## BH and the mask in one GPU call, with the original's two messages per pair.  The Wilcoxon jitter comes from the
 ## library's generator (rnorm's law, mean 1e-4, sd 1e-4), seeded by two draws of R's RNG; reference-side draws are shared by
@@ -1016,8 +1051,9 @@ infercnvb200_install <- function() {
              "i3HMM_predict_CNV_via_HMM_on_whole_tumor_samples", "scale_infercnv_expr", "smooth_by_chromosome_runmeans",
              "mask_non_DE_genes_basic", "inferCNVBayesNet", "smooth_by_chromosome_coordinates",
              "define_signif_tumor_subclusters",
-             ## an internal, dot-prefixed name: its closure is b200_.parameterize..., which the get() below finds as it is
-             ".parameterize_random_cluster_heights_smoothed_trees")
+             ## internal, dot-prefixed names: their closures are b200_.parameterize... and b200_.leiden..., which the get()
+             ## below finds as they are
+             ".parameterize_random_cluster_heights_smoothed_trees", ".leiden_seurat_preprocess_routine")
     ns <- asNamespace("infercnv")
     .icnv_env$orig <- lapply(stats::setNames(fns, fns), function(f) get(f, envir = ns))
     for (f in fns) utils::assignInNamespace(f, get(paste0("b200_", f)), ns = "infercnv")

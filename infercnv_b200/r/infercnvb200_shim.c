@@ -338,6 +338,37 @@ SEXP icnvR_knn(SEXP x, SEXP k_) {
     return ans;
 }
 
+/* .leiden_seurat_preprocess_routine's graph (R/inferCNV_tumor_subclusters.R:699-723) on the genes x cells expr: Seurat's
+ * infercnv_snn with n_features 2000, npcs 10, k.param = k.  Returns list(p (n + 1, 0-based), i (nnz, 0-based), x (nnz),
+ * singular local trend fits); the graph is symmetric, so the CSR arrays are the dgCMatrix's CSC arrays. */
+SEXP icnvR_seurat_snn(SEXP expr, SEXP k_) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], n = INTEGER(dim)[1], nnz = 0;
+    int k = Rf_asInteger(k_);
+    int rc = icnv_seurat_snn_f64(REAL(expr), G, n, NULL, n, 2000, 10, k, &nnz);
+    fail_if(rc);
+    if (nnz > 2147483647) Rf_error("infercnv_b200: the SNN graph has more entries than a dgCMatrix holds");
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 4));
+    SEXP p = Rf_allocVector(INTSXP, (R_xlen_t)(n + 1));
+    SET_VECTOR_ELT(ans, 0, p);
+    SEXP i = Rf_allocVector(INTSXP, (R_xlen_t)nnz);
+    SET_VECTOR_ELT(ans, 1, i);
+    SEXP x = Rf_allocVector(REALSXP, (R_xlen_t)nnz);
+    SET_VECTOR_ELT(ans, 2, x);
+    int64_t *rp = (int64_t *)malloc(sizeof(int64_t) * (size_t)(n + 1));
+    double st[16];
+    rc = rp ? icnv_seurat_snn_fetch(rp, INTEGER(i), REAL(x), NULL, NULL, NULL) : -7;
+    if (rc == 0) {
+        for (int64_t e = 0; e <= n; ++e) INTEGER(p)[e] = (int)rp[e];
+        rc = icnv_debug_seurat_snn(st);
+    }
+    free(rp);
+    SET_VECTOR_ELT(ans, 3, Rf_ScalarInteger(rc == 0 ? (int)st[6] : 0));
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* normalize_counts_by_seq_depth (ops.R:3064-3111); normalize_factor NA -> median of colSums */
 SEXP icnvR_normalize(SEXP expr, SEXP normalize_factor) {
     SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
@@ -683,6 +714,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_smooth_coordinates", (DL_FUNC)&icnvR_smooth_coordinates, 6},
     {"icnvR_zscore_outlier_genes", (DL_FUNC)&icnvR_zscore_outlier_genes, 2},
     {"icnvR_cluster_groups", (DL_FUNC)&icnvR_cluster_groups, 4},
+    {"icnvR_seurat_snn", (DL_FUNC)&icnvR_seurat_snn, 2},
     {NULL, NULL, 0}};
 
 void R_init_infercnvb200_shim(DllInfo *dll) {

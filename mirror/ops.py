@@ -692,6 +692,16 @@ def nn2(data, k=None) -> dict:
     return {"nn.idx": idx + 1, "nn.dists": dist}
 
 
+def leiden_seurat_preprocess_routine_graph(expr_data, k_nn=20):
+    """The graph .leiden_seurat_preprocess_routine hands to cluster_leiden (R/inferCNV_tumor_subclusters.R:699-723):
+    Seurat's infercnv_snn of the genes x cells `expr_data` (vst features, ScaleData, RunPCA(npcs = 10),
+    FindNeighbors(k.param = k_nn)), exact, as a symmetric scipy.sparse.csr_matrix.  Leiden itself stays igraph's."""
+    from scipy.sparse import csr_matrix
+    r = api.seurat_snn(expr_data, k=k_nn)
+    n = len(r.indptr) - 1
+    return csr_matrix((r.data, r.indices, r.indptr), shape=(n, n))
+
+
 def hclust(d, method: str = "complete", members=None) -> dict:
     """`hclust(d, method)` as infercnv calls it (fastcluster::hclust, imported by the reference; R/inferCNV_ops.R:262 passes
     "ward.D2" by default) on a "dist" vector such as parallelDist()'s.  Returns a dict shaped like R's "hclust" object:
