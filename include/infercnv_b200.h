@@ -273,6 +273,25 @@ ICNV_API int icnv_hclust_f64(const double *d, int64_t n, int method, int32_t *me
 /* R's order from merge: hcass2's traversal (start from the last merge, expand the first column before the second).
  * Host only, no GPU. */
 ICNV_API int icnv_hclust_order(const int32_t *merge, int64_t n, int32_t *order);
+/* icnv_hclust_f64 past its 65536 limit: the same linkage on the packed strict lower triangle - R's "dist" vector itself,
+ * 4 n (n - 1) bytes on the device instead of 8 n^2 - so n is bounded by memory alone (about 130 000 observations on an
+ * 80 GB device).  Same methods, arithmetic, tie rules and output convention: wherever both run, merge / height / order
+ * equal icnv_hclust_f64's bit for bit.  The host vector goes up in 64 MB pieces through two page-locked slabs straight into
+ * the device triangle.  Before anything is allocated, the triangle plus the linkage's scratch (8 (n + P) + 4 (6 n + P)
+ * bytes, P the power of two >= n - 1) plus 256 MB is checked against the free device memory: ICNV_E_NOMEM if it does not
+ * fit.  Centroid / median: ICNV_E_UNSUPPORTED; NaN / Inf in d: ICNV_E_NONFINITE; n < 2 or another code: ICNV_E_BAD_ARG. */
+ICNV_API int icnv_hclust_tri_f64(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order);
+/* hclust(parallelDist(t(X[keep, cells])), method) in one call, for one group of any size that fits: the distances of the
+ * listed columns of the G x C matrix X (cells: n 0-based columns, NULL: all C in order, n is then ignored) over the genes
+ * keep (n_keep 0-based rows; NULL: all G; an empty list, keep != NULL and n_keep = 0: none, so every distance is 0) are
+ * written by K10's tiles straight into the device triangle and linked there - no distance vector crosses PCIe.
+ * merge / height / order equal icnv_pairwise_dist_f64 -> icnv_hclust_tri_f64 bit for bit (and icnv_cluster_groups_f64 for
+ * a group it accepts).  Only the listed columns go to the device.  Errors as icnv_hclust_tri_f64 (the memory check also
+ * counts the uploaded columns and the gathered genes); an index out of range: ICNV_E_BAD_ARG; NaN / Inf in a used column
+ * (or an infinite distance): ICNV_E_NONFINITE. */
+ICNV_API int icnv_cluster_cells_f64(const double *X, int64_t G, int64_t C, const int32_t *keep, int64_t n_keep,
+                                    const int32_t *cells, int64_t n, int method, int32_t *merge, double *height,
+                                    int32_t *order);
 
 /* caTools::runmean(x, k) with its defaults (alg "C", endrule "mean", align "center") down every column of the G x C matrix X,
  * per row range - smooth_by_chromosome_runmeans (R/inferCNV_ops.R:2679-2704) with the chromosomes as ranges.  For a range
@@ -655,6 +674,17 @@ ICNV_API int icnv_dev_zscore_outlier_genes_f64(const double *X, int64_t G, const
 ICNV_API int icnv_dev_cluster_groups_f64(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep,
                                          int64_t n_keep, const int32_t *grp_off /*host*/, const int32_t *d_grp_idx, int n_grp,
                                          int method, int32_t *merge, double *height, void *stream);
+/* icnv_hclust_tri_f64 on a device "dist" vector (left unchanged: the linkage works on its own copy): merge / height
+ * (device), no order (icnv_hclust_order on the host copy of merge).  Synchronises `stream` once, after preparing the
+ * triangle, to report non-finite input; the linkage itself is enqueued on `stream`. */
+ICNV_API int icnv_dev_hclust_tri_f64(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream);
+/* icnv_cluster_cells_f64 on device pointers: X (column stride ldx >= G, C columns), d_keep (device; NULL: all genes),
+ * d_cells (device, n columns; NULL: all C columns, n is then ignored; a gene range - one chromosome - is X offset by its
+ * first gene with G its length), merge / height (device), no order.  With a keep list the kept rows of all C columns are
+ * gathered once (n_keep x C doubles).  Synchronises `stream` to check the indices and the distances. */
+ICNV_API int icnv_dev_cluster_cells_f64(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep,
+                                        int64_t n_keep, const int32_t *d_cells, int64_t n, int method, int32_t *merge,
+                                        double *height, void *stream);
 /* icnv_mask_non_de_f64 on device pointers: X (column stride ldx >= G), Y (ldy >= G; may be X, nullable), p_raw / p_adj
  * (G x (n_sub n_ref), nullable); the group lists are HOST arrays.  Synchronises `stream` after each gene tile (non-finite
  * check) and at the end. */

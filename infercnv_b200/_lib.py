@@ -59,6 +59,10 @@ SIGNATURES = {
     "icnv_hclust_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
     "icnv_dev_hclust_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
     "icnv_hclust_order": (c_int, [_P, c_i64, _P]),
+    "icnv_hclust_tri_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
+    "icnv_dev_hclust_tri_f64": (c_int, [_P, c_i64, c_int, _P, _P, _P]),
+    "icnv_cluster_cells_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, _P, c_i64, c_int, _P, _P, _P]),
+    "icnv_dev_cluster_cells_f64": (c_int, [_P, c_i64, c_i64, c_i64, _P, c_i64, _P, c_i64, c_int, _P, _P, _P]),
     "icnv_runmean_f64": (c_int, [_P, _P, c_i64, c_i64, _P, _P, c_int, c_int]),
     "icnv_random_tree_heights_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, c_int, c_int, ct.c_uint64, _P, _P, _P, _P]),
     "icnv_dev_random_tree_heights_f64": (c_int, [_P, c_i64, c_i64, _P, c_i64, c_int, c_int, c_int, ct.c_uint64, _P, _P, _P, _P]),

@@ -373,6 +373,41 @@ def hclust(d, method="ward.D2"):
     return merge, height, order
 
 
+# the largest n the square-matrix linkage (icnv_hclust_f64, cluster_groups) accepts; hclust_tri / cluster_cells go past it
+HCLUST_NMAX = 65536
+
+
+def hclust_tri(d, method="ward.D2"):
+    """hclust() as api.hclust returns it, on the packed triangle (icnv_hclust_tri_f64): bit-identical to api.hclust where
+    both run, and for any n whose 4 n (n - 1) bytes (plus the scratch) fit the free device memory - past HCLUST_NMAX."""
+    d = np.ascontiguousarray(d, dtype=np.float64).ravel()
+    n = _dist_size(d.size)
+    merge = np.empty((max(n - 1, 0), 2), dtype=np.int32, order="F")
+    height = np.empty(max(n - 1, 0), dtype=np.float64)
+    order = np.empty(n, dtype=np.int32)
+    _lib.check(_lib.load().icnv_hclust_tri_f64(_p(d), n, hclust_method_code(method), _p(merge), _p(height), _p(order)))
+    return merge, height, order
+
+
+def cluster_cells(X, cells=None, method="ward.D2", keep=None):
+    """hclust(parallelDist(t(X[keep, cells])), method) for one cell list (default: all columns of the genes x cells matrix X)
+    of any size that fits the device, in one call (icnv_cluster_cells_f64): (merge, height, order), bit-identical to
+    hclust_tri(pairwise_dist(X[keep], cells), method).  keep: genes to use (default all; an empty list uses none)."""
+    X = _f64(X)
+    G, C = X.shape
+    idx = None if cells is None else _i32(cells)
+    n = C if idx is None else len(idx)
+    k = None if keep is None else _i32(keep)
+    kp = np.zeros(1, np.int32) if k is not None and k.size == 0 else k   # non-NULL: "no genes", never read
+    merge = np.empty((max(n - 1, 0), 2), dtype=np.int32, order="F")
+    height = np.empty(max(n - 1, 0), dtype=np.float64)
+    order = np.empty(max(n, 1), dtype=np.int32)
+    _lib.check(_lib.load().icnv_cluster_cells_f64(
+        _p(X), G, C, _p(kp), 0 if k is None else len(k), _p(idx) if idx is not None else None, n, hclust_method_code(method),
+        _p(merge), _p(height), _p(order)))
+    return merge, height, order[:n]
+
+
 def hclust_order(merge) -> np.ndarray:
     """R's `order` from a merge matrix ((n - 1) x 2): hcass2's traversal, on the host (icnv_hclust_order)."""
     m = np.asfortranarray(merge, dtype=np.int32)

@@ -13,7 +13,7 @@ OUT = os.path.join(HERE, "libinfercnv_b200.so")
 SOURCES = ["icnv_api.cu", "icnv_smooth.cu", "icnv_viterbi.cu", "icnv_median_filter.cu", "icnv_reduce.cu",
            "icnv_synth.cu", "icnv_regions.cu", "icnv_ingest.cu", "icnv_dist.cu", "icnv_hclust.cu",
            "icnv_random_trees.cu", "icnv_de.cu", "icnv_de_multi.cu", "icnv_bayes.cu", "icnv_smooth_coords.cu",
-           "icnv_subclusters.cu", "icnv_snn.cu"]
+           "icnv_subclusters.cu", "icnv_snn.cu", "icnv_hclust_tri.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -2350,6 +2350,87 @@ int icnv_debug_cluster_groups(double *out5) {
 
 }  // extern "C"
 
+// ---- hclust on the packed triangle, K19 (kernels and device bodies in icnv_hclust_tri.cu) -----------------------------------
+// Weak references, as for the linkage: a build without icnv_hclust_tri.cu reports them as unsupported.
+namespace icnv {
+int hclust_tri_check(int64_t n, int method, const char *who) __attribute__((weak));
+int hclust_tri_room(int64_t n, size_t extra, const char *who) __attribute__((weak));
+int hclust_tri_host(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order,
+                    const char *who) __attribute__((weak));
+int hclust_tri_dev(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream,
+                   const char *who) __attribute__((weak));
+int cluster_cells_dev(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep, int64_t n_keep,
+                      const int32_t *d_cells, int64_t n, int method, int32_t *merge, double *height, void *stream,
+                      const char *who) __attribute__((weak));
+}  // namespace icnv
+
+extern "C" {
+
+int icnv_hclust_tri_f64(const double *d, int64_t n, int method, int32_t *merge, double *height, int32_t *order) {
+    static const char *who = "icnv_hclust_tri_f64";
+    if (!icnv::hclust_tri_host) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no packed-triangle linkage", who);
+    return icnv::hclust_tri_host(d, n, method, merge, height, order, who);
+}
+
+int icnv_dev_hclust_tri_f64(const double *d_dist, int64_t n, int method, int32_t *merge, double *height, void *stream) {
+    static const char *who = "icnv_dev_hclust_tri_f64";
+    if (!icnv::hclust_tri_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no packed-triangle linkage", who);
+    return icnv::hclust_tri_dev(d_dist, n, method, merge, height, stream, who);
+}
+
+int icnv_cluster_cells_f64(const double *X, int64_t G, int64_t C, const int32_t *keep, int64_t n_keep, const int32_t *cells,
+                           int64_t n, int method, int32_t *merge, double *height, int32_t *order) {
+    static const char *who = "icnv_cluster_cells_f64";
+    if (!icnv::cluster_cells_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no packed-triangle linkage", who);
+    if (!cells) n = C;
+    int rc = icnv::hclust_tri_check(n, method, who);
+    if (rc) return rc;
+    if (!X || G < 0 || C < 1 || n_keep < 0 || !merge || !height || !order || (keep && n_keep > 0 && G < 1))
+        return set_error(ICNV_E_BAD_ARG, "%s: bad argument", who);
+    for (int64_t i = 0; cells && i < n; ++i)
+        if (cells[i] < 0 || cells[i] >= C) return set_error(ICNV_E_BAD_ARG, "%s: cell index out of range", who);
+    for (int64_t i = 0; keep && i < n_keep; ++i)
+        if (keep[i] < 0 || keep[i] >= G) return set_error(ICNV_E_BAD_ARG, "%s: gene index out of range", who);
+    ICNV_HOST_PROLOGUE();
+    // everything this call will hold on the device besides the triangle, before any of it is allocated
+    const int64_t Gk = keep ? n_keep : G, nm = n - 1;
+    const size_t x_bytes = sizeof(double) * (size_t)std::max<int64_t>(G * n, 1);
+    const size_t out_bytes = (sizeof(double) + 2 * sizeof(int32_t)) * (size_t)nm;
+    const size_t extra = (x_bytes > c.slot_bytes[SLOT_IN] ? x_bytes : 0) + (out_bytes > c.slot_bytes[SLOT_OUT] ? out_bytes : 0) +
+                         (keep && Gk > 0 ? sizeof(double) * (size_t)Gk * (size_t)n : 0) + 256;
+    if ((rc = icnv::hclust_tri_room(n, extra, who))) return rc;
+    double *dX = nullptr;
+    int32_t *d_idx = nullptr, *d_keep = nullptr;
+    double *d_height = (double *)scratch(SLOT_OUT, out_bytes);
+    if (!d_height) return ICNV_E_NOMEM;
+    int32_t *d_merge = (int32_t *)(d_height + nm);
+    if (cells) {
+        if ((rc = upload_listed_columns(X, G, cells, n, &dX, &d_idx, st))) return rc;
+    } else if ((rc = upload_matrix_ring(X, G * C, &dX, st))) {
+        return rc;
+    }
+    if (keep) {   // an empty list still means "no genes": any non-NULL device pointer stands for it
+        d_keep = n_keep > 0 ? (int32_t *)scratch(SLOT_IDX2, sizeof(int32_t) * (size_t)n_keep) : d_merge;
+        if (!d_keep) return ICNV_E_NOMEM;
+        if (n_keep > 0) ICNV_CUDA(cudaMemcpyAsync(d_keep, keep, sizeof(int32_t) * (size_t)n_keep, cudaMemcpyHostToDevice, st));
+    }
+    if ((rc = icnv::cluster_cells_dev(dX, G, G, n, d_keep, n_keep, nullptr, n, method, d_merge, d_height, st, who))) return rc;
+    ICNV_CUDA(cudaMemcpyAsync(merge, d_merge, sizeof(int32_t) * 2 * (size_t)nm, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaMemcpyAsync(height, d_height, sizeof(double) * (size_t)nm, cudaMemcpyDeviceToHost, st));
+    ICNV_CUDA(cudaStreamSynchronize(st));
+    return icnv_hclust_order(merge, n, order);
+}
+
+int icnv_dev_cluster_cells_f64(const double *X, int64_t G, int64_t ldx, int64_t C, const int32_t *d_keep, int64_t n_keep,
+                               const int32_t *d_cells, int64_t n, int method, int32_t *merge, double *height, void *stream) {
+    static const char *who = "icnv_dev_cluster_cells_f64";
+    if (!icnv::cluster_cells_dev) return set_error(ICNV_E_UNSUPPORTED, "%s: this build has no packed-triangle linkage", who);
+    if (!d_cells) n = C;
+    return icnv::cluster_cells_dev(X, G, ldx, C, d_keep, n_keep, d_cells, n, method, merge, height, stream, who);
+}
+
+}  // extern "C"
+
 // ---- Seurat's SNN graph, K18 (kernels and the device body in icnv_snn.cu) ---------------------------------------------------
 // Weak references, as for the linkage: a build without icnv_snn.cu reports them as unsupported.
 namespace icnv {

@@ -30,6 +30,7 @@
 // them out.  The stable sort (bitonic on (height, raw step) in global scratch) and the conversion to R's merge matrix run
 // in the same launch.  The matrix is filled from R's condensed "dist" layout by two grid-wide kernels before it.
 #include "icnv_common.cuh"
+#include "icnv_linkage.cuh"
 
 #include <algorithm>
 
@@ -68,9 +69,6 @@ __device__ __forceinline__ void mbar_wait(void *bar, unsigned parity) {
 // generic-proxy stores to global memory (the row / column update) made visible to the bulk copies of later scans
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
 
-// total order on doubles with -0 == +0 (what a numeric comparison does): key of v + 0.0
-__device__ __forceinline__ unsigned long long dkey(double v) { return key_of(__dadd_rn(v, 0.0)); }
-
 struct HcParams {
     double *M;               // n x ld, symmetric, diagonal +inf
     int64_t n, ld;
@@ -93,24 +91,6 @@ struct HcParams {
     // are then the bases of the 8-byte and the int32 scratch)
     const HcMember *mem;
 };
-
-__device__ __forceinline__ double lance_williams(int method, double dki, double dkj, double dij, double ni, double nj,
-                                                 double nk) {
-    switch (method) {
-    case 0: return dki < dkj ? dki : dkj;
-    case 1: return dki > dkj ? dki : dkj;
-    case 2: return __ddiv_rn(__dadd_rn(__dmul_rn(ni, dki), __dmul_rn(nj, dkj)), __dadd_rn(ni, nj));
-    case 3: return __ddiv_rn(__dadd_rn(dki, dkj), 2.0);
-    default:  // 4 ward.D, 7 ward.D2 (squared input)
-        return __ddiv_rn(__dadd_rn(__dadd_rn(__dmul_rn(__dadd_rn(ni, nk), dki), __dmul_rn(__dadd_rn(nj, nk), dkj)),
-                                   -__dmul_rn(nk, dij)),
-                         __dadd_rn(__dadd_rn(ni, nj), nk));
-    }
-}
-
-__device__ __forceinline__ bool key_less(unsigned long long ka, int ia, unsigned long long kb, int ib) {
-    return ka < kb || (ka == kb && ia < ib);
-}
 
 // Condensed "dist" rows [a0, a1) -> upper triangle of M (squared for ward.D2), diagonal +inf.  src holds the entries of
 // those rows back to back (row a starts at off(a) - off(a0), off(a) = n a - a (a + 1) / 2).  flag |= 1 on NaN / Inf.
@@ -310,56 +290,8 @@ __global__ void __launch_bounds__(HC_NT, 1) hclust_nn_chain_kernel(const HcParam
         }
     }
 
-    // ---- stable sort of the raw merges by height: bitonic on (key, raw step), P = power of two >= n - 1 ----
-    const int nm = (int)(n - 1), P = p.P;
-    for (int t = tid; t < P; t += HC_NT) {
-        p.skey[t] = t < nm ? dkey(p.raw_h[t]) : ~0ull;
-        p.sidx[t] = t < nm ? t : 0x7fffffff;
-    }
-    __syncthreads();
-    for (int k = 2; k <= P; k <<= 1)
-        for (int jj = k >> 1; jj > 0; jj >>= 1) {
-            for (int t = tid; t < P; t += HC_NT) {
-                const int l = t ^ jj;
-                if (l <= t) continue;
-                const unsigned long long ka = p.skey[t], kb = p.skey[l];
-                const int ia = p.sidx[t], ib = p.sidx[l];
-                const bool up = (t & k) == 0;
-                if (up ? key_less(kb, ib, ka, ia) : key_less(ka, ia, kb, ib)) {
-                    p.skey[t] = kb; p.skey[l] = ka;
-                    p.sidx[t] = ib; p.sidx[l] = ia;
-                }
-            }
-            __syncthreads();
-        }
-    // ---- R's merge matrix: union-find over the slots in sorted order ----
-    for (int64_t k = tid; k < n; k += HC_NT) {
-        p.uf[k] = (int32_t)k;
-        p.node[k] = (int32_t)k;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        auto find = [&](int x) {
-            while (p.uf[x] != x) {
-                const int gp = p.uf[p.uf[x]];
-                p.uf[x] = gp;
-                x = gp;
-            }
-            return x;
-        };
-        for (int s = 0; s < nm; ++s) {
-            const int t = p.sidx[s];
-            const int x = find(p.raw_i[t]), y = find(p.raw_j[t]);
-            const int nx = p.node[x], ny = p.node[y];
-            const int lo = nx < ny ? nx : ny, hi = nx < ny ? ny : nx;
-            p.merge[s] = lo < n ? -(lo + 1) : lo - (int)n + 1;
-            p.merge[nm + s] = hi < n ? -(hi + 1) : hi - (int)n + 1;
-            const double h = p.raw_h[t];
-            p.height[s] = p.method == 7 ? sqrt(h) : h;
-            p.uf[x] = y;
-            p.node[y] = (int)n + s;
-        }
-    }
+    // ---- stable sort of the raw merges by height, then R's merge matrix ----
+    linkage_finish<HC_NT>(n, p.method, p.P, p.raw_h, p.raw_i, p.raw_j, p.skey, p.sidx, p.uf, p.node, p.merge, p.height);
 }
 
 }  // namespace hc

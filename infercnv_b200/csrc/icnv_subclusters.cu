@@ -93,7 +93,7 @@ __global__ void __launch_bounds__(256) index_check_kernel(const int32_t *__restr
     if (bad) atomicOr(flag, 2);
 }
 
-static int check_indices(const int32_t *d_idx, int64_t n, int64_t lim, int *flag, cudaStream_t st) {
+int check_indices(const int32_t *d_idx, int64_t n, int64_t lim, int *flag, cudaStream_t st) {
     if (n <= 0) return ICNV_OK;
     const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 1024);
     index_check_kernel<<<grid, 256, 0, st>>>(d_idx, n, lim, flag);

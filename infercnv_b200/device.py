@@ -442,6 +442,45 @@ class Engine:
         m = merge.cpu().numpy().T
         return m, height.cpu().numpy(), hclust_order(m)
 
+    def hclust_tri(self, D, n, method="ward.D2"):
+        """Engine.hclust on the packed triangle (icnv_dev_hclust_tri_f64): any n that fits the device, bit-identical to
+        Engine.hclust where both run.  D is left unchanged."""
+        from .api import hclust_method_code, hclust_order
+        if D.dtype != torch.float64 or not D.is_contiguous() or D.numel() != n * (n - 1) // 2:
+            raise ValueError("D must be a contiguous float64 device vector of n (n - 1) / 2 entries")
+        merge = torch.empty((2, max(n - 1, 0)), dtype=torch.int32, device=self.tdev)   # column-major (n - 1) x 2
+        height = torch.empty(max(n - 1, 0), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_hclust_tri_f64(D.data_ptr(), n, hclust_method_code(method), merge.data_ptr(),
+                                                    height.data_ptr(), _stream_ptr()))
+        m = merge.cpu().numpy().T
+        return m, height.cpu().numpy(), hclust_order(m)
+
+    def cluster_cells(self, X, cells=None, method="ward.D2", keep=None):
+        """api.cluster_cells on the listed local cells (rows of X; default all) on the device: X is a (C, G) float64 tensor
+        with contiguous genes, or a gene-range view of one (X[:, a:b], one chromosome), as Engine.knn takes it.  keep: gene
+        indices within X's columns (host list or device tensor).  Returns (merge, height, order) as numpy arrays; no
+        distance vector leaves the device."""
+        from .api import hclust_method_code, hclust_order
+        if X.dtype != torch.float64 or X.dim() != 2 or (X.shape[1] > 1 and X.stride(1) != 1):
+            raise ValueError("X must be a (cells, genes) float64 tensor with contiguous genes")
+        C, G = X.shape
+        idx = None if cells is None else torch.as_tensor(np.asarray(cells, dtype=np.int32), device=self.tdev)
+        n = C if idx is None else int(idx.numel())
+        d_keep = None
+        if keep is not None:
+            d_keep = torch.as_tensor(np.asarray(keep.cpu() if torch.is_tensor(keep) else keep, dtype=np.int32), device=self.tdev)
+        n_keep = 0 if d_keep is None else int(d_keep.numel())
+        if d_keep is not None and n_keep == 0:
+            d_keep = torch.zeros(1, dtype=torch.int32, device=self.tdev)   # non-NULL: "no genes", never read
+        merge = torch.empty((2, max(n - 1, 0)), dtype=torch.int32, device=self.tdev)   # column-major (n - 1) x 2
+        height = torch.empty(max(n - 1, 0), dtype=torch.float64, device=self.tdev)
+        _lib.check(self.lib.icnv_dev_cluster_cells_f64(
+            X.data_ptr(), G, max(X.stride(0), G), C, None if d_keep is None else d_keep.data_ptr(), n_keep,
+            idx.data_ptr() if idx is not None else None, n, hclust_method_code(method), merge.data_ptr(), height.data_ptr(),
+            _stream_ptr()))
+        m = merge.cpu().numpy().T
+        return m, height.cpu().numpy(), hclust_order(m)
+
     def random_tree_heights(self, X, cells=None, window=101, method="ward.D2", n_perm=100, seed=0):
         """The random-trees permutation null of the clade `cells` (rows of the resident (C, G) float64 tensor X with
         contiguous genes; default all) on the device: (merge, height, order, perm_max) as numpy arrays, as

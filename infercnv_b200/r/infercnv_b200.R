@@ -445,7 +445,7 @@ infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_c
 b200_parallelDist <- function(x, method = "euclidean", diag = FALSE, upper = FALSE, threads = NULL, ...) {
     orig <- .icnv_env$orig_parallelDist
     ok <- .icnv_enabled() && identical(method, "euclidean") && is.matrix(x) && is.double(x) && !anyNA(x) && nrow(x) >= 2 &&
-        nrow(x) <= 65536          # hclust()'s own limit
+        nrow(x) <= 65535 * 128    # the distance kernel's tile grid; hclust() past 65 536 takes the packed-triangle linkage
     if (ok) {
         d <- .icnv_try(.Call("icnvR_pairwise_dist", x), "parallelDist (euclidean)")
         if (!is.null(d)) {
@@ -460,18 +460,21 @@ b200_parallelDist <- function(x, method = "euclidean", diag = FALSE, upper = FAL
 ## fastcluster::hclust as infercnv calls it on every parallelDist() result - hclust(d, method = hclust_method), default
 ## "ward.D2" (R/inferCNV_ops.R:262; R/inferCNV_tumor_subclusters.R:191,411,474,498,582,609; R/inferCNV_ops.R:1930,3242;
 ## R/inferCNV_heatmap.R:719,755,1062,1079).  Same signature as fastcluster::hclust(d, method = "complete", members = NULL)
-## and the same "hclust" object.  The six reducible methods run as a nearest-neighbour chain on the GPU; anything else - not
-## a "dist", non-NULL members, centroid / median / the alias "ward", fewer than 2 or more than 65 536 observations, NA in
-## d, or a library error - goes to the original.
+## and the same "hclust" object.  The six reducible methods run as a nearest-neighbour chain on the GPU: up to 65 536
+## observations on the square matrix (icnvR_hclust), beyond that on the packed triangle (icnvR_hclust_tri, the same tree
+## bit for bit, bounded by the free device memory: 4 n (n - 1) bytes plus scratch).  Anything else - not a "dist", non-NULL
+## members, centroid / median / the alias "ward", fewer than 2 observations, NA in d, or a library error (a triangle that
+## does not fit is ICNV_E_NOMEM) - goes to the original, with the error logged.
 b200_hclust <- function(d, method = "complete", members = NULL) {
     orig <- .icnv_env$orig_hclust
     codes <- c(single = 0L, complete = 1L, average = 2L, mcquitty = 3L, ward.D = 4L, ward.D2 = 7L)
     n <- if (inherits(d, "dist")) attr(d, "Size") else NA
     ok <- .icnv_enabled() && inherits(d, "dist") && is.null(members) && is.character(method) && length(method) == 1 &&
-        method %in% names(codes) && !is.null(n) && !is.na(n) && n >= 2 && n <= 65536 && !anyNA(d)
+        method %in% names(codes) && !is.null(n) && !is.na(n) && n >= 2 && !anyNA(d)
     if (ok) {
         code <- codes[[method]]
-        res <- .icnv_try(.Call("icnvR_hclust", d, code), "hclust")
+        res <- if (n <= 65536) .icnv_try(.Call("icnvR_hclust", d, code), "hclust") else
+            .icnv_try(.Call("icnvR_hclust_tri", d, code), "hclust (packed triangle)")
         if (!is.null(res)) {
             return(structure(list(merge = res[[1]], height = res[[2]], order = res[[3]], labels = attr(d, "Labels"),
                                   method = method, call = match.call(), dist.method = attr(d, "method")),
@@ -853,8 +856,7 @@ b200_define_signif_tumor_subclusters <- function(infercnv_obj, p_val = 0.1, k_nn
     }
     ok <- .icnv_enabled() && !isTRUE(restrict_to_DE_genes) && .icnv_ok(m) && nrow(m) >= 2 && is.character(hclust_method) &&
         length(hclust_method) == 1 && hclust_method %in% names(codes) && is.character(partition_method) &&
-        length(partition_method) == 1 && partition_method %in% c("leiden", "qnorm", "pheight", "qgamma", "none") &&
-        all(lengths(tumor_groups) <= 65536)
+        length(partition_method) == 1 && partition_method %in% c("leiden", "qnorm", "pheight", "qgamma", "none")
     if (!ok) return(call_orig())
     leiden_method <- match.arg(leiden_method)
     leiden_method_per_chr <- match.arg(leiden_method_per_chr)
@@ -876,10 +878,26 @@ b200_define_signif_tumor_subclusters <- function(infercnv_obj, p_val = 0.1, k_nn
         structure(list(merge = tr[[1]], height = tr[[2]], order = tr[[3]], labels = colnames(m)[cols], method = hclust_method,
                        call = match.call(), dist.method = "euclidean"), class = "hclust")
     }
+    ## groups of up to 65 536 cells in one icnvR_cluster_groups call; each larger one through icnvR_cluster_cells (the
+    ## packed-triangle linkage, bounded by the free device memory); the same trees either way
     trees_of <- function(lists) {
         if (length(lists) == 0) return(list())
-        .icnv_try(.Call("icnvR_cluster_groups", m, if (is.null(keep)) NULL else as.integer(keep),
-                        lapply(lists, as.integer), codes[[hclust_method]]), "subcluster trees")
+        kp <- if (is.null(keep)) NULL else as.integer(keep)
+        big <- lengths(lists) > 65536
+        out <- vector("list", length(lists))
+        if (any(!big)) {
+            small <- .icnv_try(.Call("icnvR_cluster_groups", m, kp, lapply(lists[!big], as.integer), codes[[hclust_method]]),
+                               "subcluster trees")
+            if (is.null(small)) return(NULL)
+            out[!big] <- small
+        }
+        for (i in which(big)) {
+            tr <- .icnv_try(.Call("icnvR_cluster_cells", m, kp, as.integer(lists[[i]]), codes[[hclust_method]]),
+                            "subcluster tree (more than 65 536 cells)")
+            if (is.null(tr)) return(NULL)
+            out[[i]] <- tr
+        }
+        out
     }
 
     res <- list()

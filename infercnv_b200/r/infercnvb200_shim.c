@@ -257,6 +257,24 @@ SEXP icnvR_hclust(SEXP d, SEXP method_code) {
     return ans;
 }
 
+/* hclust(d, method) past 65 536 observations: the packed-triangle linkage on R's "dist" vector as it is. */
+SEXP icnvR_hclust_tri(SEXP d, SEXP method_code) {
+    R_xlen_t len = Rf_xlength(d);
+    int64_t n = (int64_t)((1.0 + sqrt(1.0 + 8.0 * (double)len)) / 2.0 + 0.5);
+    if (n * (n - 1) / 2 != (int64_t)len || n < 2) Rf_error("infercnv_b200: not a \"dist\" vector of at least 2 observations");
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 3));
+    SEXP merge = Rf_allocMatrix(INTSXP, (int)(n - 1), 2);
+    SET_VECTOR_ELT(ans, 0, merge);
+    SEXP height = Rf_allocVector(REALSXP, (R_xlen_t)(n - 1));
+    SET_VECTOR_ELT(ans, 1, height);
+    SEXP order = Rf_allocVector(INTSXP, (R_xlen_t)n);
+    SET_VECTOR_ELT(ans, 2, order);
+    int rc = icnv_hclust_tri_f64(REAL(d), n, Rf_asInteger(method_code), INTEGER(merge), REAL(height), INTEGER(order));
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 /* apply(m, 2, caTools::runmean, k = k) per row range - smooth_by_chromosome_runmeans (ops.R:2679-2704) with the ranges the
  * R closure computed (0-based starts, lengths; genes outside them are copied). */
 SEXP icnvR_runmean(SEXP expr, SEXP chr_start, SEXP chr_len, SEXP k) {
@@ -694,6 +712,38 @@ SEXP icnvR_cluster_groups(SEXP expr, SEXP keep, SEXP groups, SEXP method_code) {
 
 SEXP icnvR_available(void) { return Rf_ScalarLogical(icnv_device_count() > 0 && icnv_init(-1) == 0); }
 
+/* hclust(parallelDist(t(expr[keep, cells])), method) for one group of any size that fits the device: keep (1-based rows or
+ * NULL = all; integer(0) = none), cells (1-based columns) -> list(merge, height, order). */
+SEXP icnvR_cluster_cells(SEXP expr, SEXP keep, SEXP cells, SEXP method_code) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int64_t n = Rf_length(cells), n_keep = Rf_isNull(keep) ? 0 : Rf_length(keep);
+    if (n < 2) Rf_error("infercnv_b200: a tree needs at least 2 cells");
+    int32_t *kp = (int32_t *)malloc(sizeof(int32_t) * (size_t)(n_keep > 0 ? n_keep : 1));
+    int32_t *cl = (int32_t *)malloc(sizeof(int32_t) * (size_t)n);
+    if (!kp || !cl) {
+        free(kp);
+        free(cl);
+        Rf_error("infercnv_b200: out of host memory");
+    }
+    for (int64_t i = 0; i < n_keep; ++i) kp[i] = INTEGER(keep)[i] - 1;
+    for (int64_t i = 0; i < n; ++i) cl[i] = INTEGER(cells)[i] - 1;
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 3));
+    SEXP merge = Rf_allocMatrix(INTSXP, (int)(n - 1), 2);
+    SET_VECTOR_ELT(ans, 0, merge);
+    SEXP height = Rf_allocVector(REALSXP, (R_xlen_t)(n - 1));
+    SET_VECTOR_ELT(ans, 1, height);
+    SEXP order = Rf_allocVector(INTSXP, (R_xlen_t)n);
+    SET_VECTOR_ELT(ans, 2, order);
+    int rc = icnv_cluster_cells_f64(REAL(expr), G, C, Rf_isNull(keep) ? NULL : kp, n_keep, cl, n, Rf_asInteger(method_code),
+                                    INTEGER(merge), REAL(height), INTEGER(order));
+    free(kp);
+    free(cl);
+    UNPROTECT(1);
+    fail_if(rc);
+    return ans;
+}
+
 static const R_CallMethodDef call_methods[] = {
     {"icnvR_subtract_ref", (DL_FUNC)&icnvR_subtract_ref, 4}, {"icnvR_smooth", (DL_FUNC)&icnvR_smooth, 3},
     {"icnvR_center", (DL_FUNC)&icnvR_center, 2},             {"icnvR_smooth_block", (DL_FUNC)&icnvR_smooth_block, 7},
@@ -714,6 +764,8 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_smooth_coordinates", (DL_FUNC)&icnvR_smooth_coordinates, 6},
     {"icnvR_zscore_outlier_genes", (DL_FUNC)&icnvR_zscore_outlier_genes, 2},
     {"icnvR_cluster_groups", (DL_FUNC)&icnvR_cluster_groups, 4},
+    {"icnvR_hclust_tri", (DL_FUNC)&icnvR_hclust_tri, 2},
+    {"icnvR_cluster_cells", (DL_FUNC)&icnvR_cluster_cells, 4},
     {"icnvR_seurat_snn", (DL_FUNC)&icnvR_seurat_snn, 2},
     {NULL, NULL, 0}};
 

@@ -709,8 +709,21 @@ def hclust(d, method: str = "complete", members=None) -> dict:
     on the GPU."""
     if members is not None:
         raise NotImplementedError("hclust(members=...) is not on the GPU path")
-    merge, height, order = api.hclust(d, method)
+    d = np.ascontiguousarray(d, dtype=np.float64).ravel()
+    big = d.size > api.HCLUST_NMAX * (api.HCLUST_NMAX - 1) // 2   # past the square matrix: the packed-triangle linkage
+    merge, height, order = (api.hclust_tri if big else api.hclust)(d, method)
     return {"merge": merge, "height": height, "order": order, "labels": None, "method": method, "dist.method": "euclidean"}
+
+
+def cluster_groups(expr_data, groups, method: str = "ward.D2", keep=None) -> list:
+    """`hclust(parallelDist(t(expr_data[keep, g])), method)` for every cell list g of `groups`, as (merge, height, order) in
+    group order: the groups of at most api.HCLUST_NMAX cells in one api.cluster_groups call, each larger one through
+    api.cluster_cells (the packed-triangle linkage, bounded by device memory).  Both return the same bits where both run."""
+    big = [len(g) > api.HCLUST_NMAX for g in groups]
+    small = [g for g, b in zip(groups, big) if not b]
+    small = api.cluster_groups(expr_data, small, method=method, keep=keep) if small else []
+    it = iter(small)
+    return [api.cluster_cells(expr_data, g, method=method, keep=keep) if b else next(it) for g, b in zip(groups, big)]
 
 
 def runmean(x, k) -> np.ndarray:
@@ -785,7 +798,8 @@ def define_signif_tumor_subclusters(infercnv_obj: Infercnv, p_val: float = 0.1, 
     """define_signif_tumor_subclusters (R/inferCNV_tumor_subclusters.R:2-177) for partition_method "none", "pheight" and
     "qnorm": returns (infercnv_obj with tumor_subclusters = {"hc": {group: hclust dict or None}, "subclusters": {group:
     {"<group>_s<id>": indices}}}, None), the hidden spike mirrored with partition_method "none".  The z-score gene filter
-    (icnv_zscore_outlier_genes_f64) and every group's tree (icnv_cluster_groups_f64) are two GPU calls; the cut heights and
+    (icnv_zscore_outlier_genes_f64) and every group's tree (icnv_cluster_groups_f64; a group above 65 536 cells through
+    icnv_cluster_cells_f64) are GPU calls; the cut heights and
     cutree() are host arithmetic on the returned trees, as in R.  "qgamma" (fitdistrplus) and "leiden" (igraph's RNG) are not
     on this path, nor is restrict_to_DE_genes."""
     if partition_method in ("leiden", "qgamma"):
@@ -812,8 +826,7 @@ def define_signif_tumor_subclusters(infercnv_obj: Infercnv, p_val: float = 0.1, 
             keep = keep[:0]
     names = list(tumor_groups)
     treed = [g for g in names if len(tumor_groups[g]) > 2]
-    trees = dict(zip(treed, api.cluster_groups(obj.expr_data, [tumor_groups[g] for g in treed], method=hclust_method,
-                                               keep=keep)))
+    trees = dict(zip(treed, cluster_groups(obj.expr_data, [tumor_groups[g] for g in treed], method=hclust_method, keep=keep)))
     res = {"hc": {}, "subclusters": {}}
     for g in names:
         log.info("define_signif_tumor_subclusters(), tumor: %s", g)
