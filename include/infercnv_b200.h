@@ -182,6 +182,34 @@ ICNV_API int icnv_smooth_hmm_u8_f64(const double *X, double *Y, uint8_t *states,
                                     int use_bounds, int m, const double *Pi, const double *delta, const double *mean,
                                     const double *sd);
 
+/* The i3 counterpart, with the median filter on the same pass: run() steps 4..14, the i3 model, step 17 per cell and
+ * apply_median_filtering, for HMM_type = "i3", analysis_mode = "cells", use_KS = FALSE.  The matrix is read once and
+ * every output written once.
+ *   Y       = icnv_smooth_block_f64 with the same arguments (bit-identical).
+ *   model   = {mu, sigma, mean_delta}: mu and sigma over every value of the reference cells in Y
+ *             (.i3HMM_get_sd_trend_by_num_cells_fit, R/inferCNV_i3HMM.R:17-80; bit-identical to icnv_mean_sd_f64(Y,
+ *             grp_idx)), mean_delta = |qnorm(i3_p_val, 0, sigma)| (Wichura's AS241, as R's qnorm).  They are fixed
+ *             from the reference cells before the first observation cell is processed.
+ *   states  = per-cell icnv_viterbi_u8_f64 of Y under .i3HMM_get_HMM (i3HMM.R:99-156): transition diagonal 1 - 5t,
+ *             off-diagonal t, delta (t, 1 - 5t, t), means (mu - d, mu, mu + d), sd sigma.
+ *   F       = icnv_median_filter_f64(Y, mf lists, mf_window) (noise_reduction.R:43-113; cells in no list are copied,
+ *             so n_mf == 0 gives F = Y); F == NULL: no filter, mf_* and mf_window are not read.  The cells are cut
+ *             into runs no list's span crosses; one run's Y and F (2 x 8 x G bytes per cell of it) stay on the device
+ *             at a time, and a run that does not fit is ICNV_E_NOMEM before any output is written.  The two buffers
+ *             stay allocated at the largest run's size until icnv_shutdown / icnv_init, like the library's other
+ *             scratch: lists whose spans overlap across a large group make that run, and the buffers, large.  Lists
+ *             may be arbitrary column sets.
+ * Several devices (icnv_init_devices): the cells are cut at the run boundaries nearest to even shares; every device
+ * allocates its buffers before any device starts, so the ICNV_E_NOMEM above still leaves every output unwritten;
+ * every device reduces all reference cells itself, so every output is independent of the device count.
+ * BAD_ARG: an even window, an even mf_window or mf_window < 3 (with F), an index out of range, i3_p_val outside
+ * (0, 1), G < 2. */
+ICNV_API int icnv_smooth_i3_hmm_u8_f64(const double *X, double *Y, uint8_t *states, double *F, int64_t G, int64_t C,
+                                       const int32_t *chr_start, const int32_t *chr_len, int K, const int32_t *grp_off,
+                                       const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window,
+                                       int use_bounds, double i3_p_val, double t, const int32_t *mf_off,
+                                       const int32_t *mf_idx, int n_mf, int mf_window, double *model);
+
 /* Viterbi.dthmm.adj, R/inferCNV_HMM.R:1101-1176, batched over the drivers
  * predict_CNV_via_HMM_on_indiv_cells (HMM.R:284-324), ..._on_tumor_subclusters (:345-408),
  * ..._on_whole_tumor_samples (:509-567) and the i3 twins (R/inferCNV_i3HMM.R:180-389).

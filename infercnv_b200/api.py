@@ -220,6 +220,28 @@ def smooth_hmm(X, chr_start, chr_len, ref_groups, Pi, delta, mean, sd, apply_log
     return Y, S
 
 
+def smooth_i3_hmm(X, chr_start, chr_len, ref_groups, i3_p_val=0.05, t=1e-6, median_lists=None, median_window=7,
+                  apply_log=True, threshold=3.0, window_length=101, use_bounds=True):
+    """Fused i3 pass (icnv_smooth_i3_hmm_u8_f64): smooth block, the i3 model of the reference cells' smoothed values,
+    per-cell i3 HMM and, with `median_lists`, apply_median_filtering(window = median_window) over those index lists, in one
+    pass over the matrix.  Returns (Y, states uint8, F or None, {"mu", "sigma", "mean_delta"})."""
+    X = _f64(X)
+    G, C = X.shape
+    cs, cl = _i32(chr_start), _i32(chr_len)
+    off, idx = groups_to_csr(ref_groups)
+    Y = np.empty_like(X, order="F")
+    S = np.empty((G, C), dtype=np.uint8, order="F")
+    lists = [] if median_lists is None else list(median_lists)
+    moff, midx = groups_to_csr(lists)
+    F = np.empty_like(X, order="F") if median_lists is not None else None
+    model = np.zeros(3, dtype=np.float64)
+    _lib.check(_lib.load().icnv_smooth_i3_hmm_u8_f64(_p(X), _p(Y), _p(S), _p(F), G, C, _p(cs), _p(cl), len(cs), _p(off), _p(idx),
+                                                     len(ref_groups), int(bool(apply_log)), float(threshold), int(window_length),
+                                                     int(bool(use_bounds)), float(i3_p_val), float(t), _p(moff), _p(midx),
+                                                     len(lists), int(median_window), _p(model)))
+    return Y, S, F, {"mu": float(model[0]), "sigma": float(model[1]), "mean_delta": float(model[2])}
+
+
 def viterbi(X, chr_start, chr_len, Pi, delta, mean, sd, groups=None, want_margins=False, out=None):
     """States (G, C): int32 with -1 = unassigned by default; a uint8 `out` selects the one-byte wire format
     (icnv_viterbi_u8_f64, 255 = unassigned)."""

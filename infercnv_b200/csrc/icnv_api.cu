@@ -357,7 +357,7 @@ static void free_slot(Ctx &c) {
         c.slot_ptr[s] = nullptr;
         c.slot_bytes[s] = 0;
     }
-    for (int i = 0; i < 6; ++i) {
+    for (int i = 0; i < 8; ++i) {
         if (c.pin_ptr[i]) cudaFreeHost(c.pin_ptr[i]);
         c.pin_ptr[i] = nullptr;
         c.pin_bytes[i] = 0;
@@ -688,31 +688,126 @@ struct HmmModel {
     const double *Pi, *delta, *mean, *sd;
 };
 
+/* qnorm(p, mu, sigma) for 0 < p < 1: Wichura's AS241 (PPND16), the algorithm of R's qnorm, with the published
+ * coefficients in the order of operations of Python's NormalDist.inv_cdf (hmm.i3_mean_delta gives the same bits). */
+static double qnorm_as241(double p, double mu, double sigma) {
+    const double q = p - 0.5;
+    double r, val;
+    if (std::fabs(q) <= .425) {
+        r = .180625 - q * q;
+        val = q * (((((((r * 2509.0809287301226727 + 33430.575583588128105) * r + 67265.770927008700853) * r +
+                        45921.953931549871457) * r + 13731.693765509461125) * r + 1971.5909503065514427) * r +
+                     133.14166789178437745) * r + 3.387132872796366608) /
+              (((((((r * 5226.4952788528545610 + 28729.085735721942674) * r + 39307.89580009271061) * r +
+                   21213.794301586595867) * r + 5394.1960214247511077) * r + 687.1870074920579083) * r +
+                42.313330701600911252) * r + 1.);
+        return mu + sigma * val;
+    }
+    r = std::sqrt(-std::log(q < 0 ? p : 1. - p));
+    if (r <= 5.) {
+        r += -1.6;
+        val = (((((((r * 7.7454501427834140764e-4 + .0227238449892691845833) * r + .24178072517745061177) * r +
+                   1.27045825245236838258) * r + 3.64784832476320460504) * r + 5.7694972214606914055) * r +
+                4.6303378461565452959) * r + 1.42343711074968357734) /
+              (((((((r * 1.05075007164441684324e-9 + 5.475938084995344946e-4) * r + .0151986665636164571966) * r +
+                   .14810397642748007459) * r + .68976733498510000455) * r + 1.6763848301838038494) * r +
+                2.05319162663775882187) * r + 1.);
+    } else {
+        r += -5.;
+        val = (((((((r * 2.01033439929228813265e-7 + 2.71155556874348757815e-5) * r + .0012426609473880784386) * r +
+                   .026532189526576123093) * r + .29656057182850489123) * r + 1.7848265399172913358) * r +
+                5.4637849111641143699) * r + 6.6579046435011037772) /
+              (((((((r * 2.04426310338993978564e-15 + 1.4215117583164458887e-7) * r + 1.8463183175100546818e-5) * r +
+                   7.868691311456132591e-4) * r + .0148753612908506148525) * r + .13692988092273580531) * r +
+                .59983220655588793769) * r + 1.);
+    }
+    if (q < 0.0) val = -val;
+    return mu + sigma * val;
+}
+
+/* What the fused i3 call adds to the slab pipeline: the i3 model, fixed from the reference cells' final values between
+ * the reference pre-pass and the first slab, and the median filter over index lists.  With the filter, the cells are cut
+ * into units - runs of columns no list's span crosses, at least a slab long - and a unit's Y stays on the device until its
+ * last slab is done; the filter then runs on the whole unit and F leaves behind it. */
+struct I3Fused {
+    double p_val, t;
+    double *model;                       // out: mu, sigma, mean_delta (NULL: this device does not report them)
+    double *F;                           // median-filtered Y; NULL: no filter
+    const int32_t *mf_off, *mf_idx;
+    int n_mf, mf_window;
+    std::vector<std::pair<int64_t, int64_t>> spans;   // merged [lo, hi) column spans of the lists, ascending
+    // the smallest column >= x that no span crosses
+    int64_t cut_at_or_after(int64_t x) const {
+        auto it = std::upper_bound(spans.begin(), spans.end(), std::make_pair(x, INT64_MAX));
+        if (it != spans.begin() && std::prev(it)->first < x && x < std::prev(it)->second) return std::prev(it)->second;
+        return x;
+    }
+    // the column nearest x that no span crosses (ties: the lower one)
+    int64_t cut_near(int64_t x) const {
+        auto it = std::upper_bound(spans.begin(), spans.end(), std::make_pair(x, INT64_MAX));
+        if (it != spans.begin() && std::prev(it)->first < x && x < std::prev(it)->second) {
+            const int64_t a = std::prev(it)->first, b = std::prev(it)->second;
+            return (x - a <= b - x) ? a : b;
+        }
+        return x;
+    }
+};
+
+// Several devices: every device's range allocates its buffers first and waits here for the others, so that a range whose
+// buffers do not fit stops every device before any of them has written output.
+struct StartGate {
+    std::mutex mu;
+    std::condition_variable cv;
+    int left;
+    bool ok = true;
+    int first_fail = -1;               // the device whose own failure closed the gate
+    std::vector<char> in;
+    StartGate(int n_dev, int n_threads) : left(n_threads), in((size_t)n_dev, 0) {}
+    // device d has allocated (good) or failed; returns whether every device may start.  A second arrival returns at once.
+    bool arrive(int d, bool good) {
+        std::unique_lock<std::mutex> lk(mu);
+        if (in[(size_t)d]) return ok;
+        in[(size_t)d] = 1;
+        if (!good && first_fail < 0) first_fail = d;
+        ok = ok && good;
+        if (--left == 0) cv.notify_all();
+        else cv.wait(lk, [&] { return left == 0; });
+        return ok;
+    }
+};
+
 // Y (optional) = smooth block of X; states (optional) = per-cell Viterbi of the block's output (or of X
 // itself when do_smooth == 0).
 // states (int32, -1 = unassigned) or states8 (uint8, 255 = unassigned): at most one of them is non-NULL.
 // Works on the cells [c_lo, c_hi) of the G x C host matrices on the calling thread's device context; the reference
 // groups index the whole matrix (every device reduces all reference cells itself, in list order).
+// i3 (with do_smooth, hmm == NULL): the per-cell HMM uses the i3 model of the block's reference cells, and F (optional)
+// is the median filter of Y; [c_lo, c_hi) must not cut a list's span.
 static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *states, uint8_t *states8, int64_t G, int64_t c_lo,
                                int64_t c_hi, const int32_t *chr_start, const int32_t *chr_len, int K, int do_smooth,
                                const int32_t *grp_off, const int32_t *grp_idx, int n_grp, int apply_log, double threshold,
-                               int window, int use_bounds, const HmmModel *hmm, CopyPool *pool) {
+                               int window, int use_bounds, const HmmModel *hmm, CopyPool *pool, const I3Fused *i3 = nullptr,
+                               StartGate *gate = nullptr) {
     cudaStream_t sc = c.stream, sh = c.s_h2d, sd = c.s_d2h;
     int rc;
     const int64_t C = c_hi - c_lo;
+    const bool mf = i3 && i3->F;
+    const bool has_hmm = hmm || i3;
     int *d_flag = (int *)scratch(SLOT_MISC, 64);
     if (!d_flag) return ICNV_E_NOMEM;
+    if (mf) d_flag += 4;   // icnv_dev_median_filter_f64 clears and sets the slot's first word for itself
     ICNV_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), sc));
     double *lo1 = nullptr, *hi1 = nullptr, *mid1 = nullptr, *lo2 = nullptr, *hi2 = nullptr, *mid2 = nullptr;
     // page-locked caller memory goes over PCIe directly; anything else through the pinned ring (pool != NULL)
     const bool stage_in = pool && !is_pinned(X);
-    const bool stage_out = pool && ((Y && !is_pinned(Y)) || (states && !is_pinned(states)) || (states8 && !is_pinned(states8)));
+    const bool stage_out = pool && ((Y && !is_pinned(Y)) || (states && !is_pinned(states)) || (states8 && !is_pinned(states8)) ||
+                                    (mf && !is_pinned(i3->F)));
 
     // ---- slabs ------------------------------------------------------------------------------------------
     // Fill and drain of the copy pipeline cost one slab each way.  Without the HMM a slab's kernel time (~0.05 ms per 256
     // cells) is far below its PCIe time (0.37 ms), so small slabs only shorten fill / drain; the per-cell Viterbi is bounded
     // below by its longest chromosome's serial recursion whatever the slab size, so HMM calls keep the measured 1024.
-    int64_t slab_cells = hmm ? SLAB_CELLS : SLAB_CELLS_SMOOTH;
+    int64_t slab_cells = has_hmm ? SLAB_CELLS : SLAB_CELLS_SMOOTH;
     if (stage_in || stage_out) {
         // pageable caller memory: fewer, larger hand-overs to the copy threads - about 320 MB of input per slab (4000 cells at
         // 10 000 genes), but at least ten slabs so that filling and draining the pipeline stays a small share
@@ -724,20 +819,45 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     if (c.opt_slab_cells) slab_cells = c.opt_slab_cells;
     const int64_t slab = std::max<int64_t>(1, std::min<int64_t>(slab_cells, C));
     const size_t slab_elems = (size_t)G * (size_t)slab;
+    // slab i is the cells [c_lo + s_at[i], c_lo + s_at[i + 1]).  With the median filter the slabs are cut inside units (see
+    // I3Fused); unit_lo[i] is the first cell of slab i's unit, unit_end[i] marks its last slab.
+    std::vector<int64_t> s_at{0}, unit_lo;
+    std::vector<char> unit_end;
+    int64_t max_unit = 0;
+    for (int64_t u0 = 0; u0 < C;) {
+        const int64_t u1 = mf ? std::min(C, i3->cut_at_or_after(c_lo + u0 + slab) - c_lo) : C;
+        for (int64_t s = u0; s < u1; s += slab) {
+            s_at.push_back(std::min(u1, s + slab));
+            unit_lo.push_back(u0);
+            unit_end.push_back(s + slab >= u1);
+        }
+        max_unit = std::max(max_unit, u1 - u0);
+        u0 = u1;
+    }
     double *dIn[2], *dOut[2] = {nullptr, nullptr};
     uint8_t *dSt[2] = {nullptr, nullptr};
     int32_t *dW[2] = {nullptr, nullptr};
-    double *pIn[2] = {nullptr, nullptr}, *pOut[2] = {nullptr, nullptr};
+    double *pIn[2] = {nullptr, nullptr}, *pOut[2] = {nullptr, nullptr}, *pF[2] = {nullptr, nullptr};
     void *pSt[2] = {nullptr, nullptr};
     const size_t st_elem = states ? sizeof(int32_t) : 1;
+    // the median filter's unit buffers (Y and F of the unit) take the place of the two output slabs
+    double *dYu = nullptr, *dFu = nullptr;
+    if (mf) {
+        const size_t unit_bytes = sizeof(double) * (size_t)G * (size_t)max_unit;
+        dYu = (double *)scratch(SLOT_SLAB_OUT0, unit_bytes);
+        dFu = dYu ? (double *)scratch(SLOT_SLAB_OUT1, unit_bytes) : nullptr;
+        if (!dYu || !dFu)
+            return set_error(ICNV_E_NOMEM, "median filter: a run of %lld cells that no index list's span crosses needs 2 x %zu "
+                             "bytes on device %d: %s", (long long)max_unit, unit_bytes, c.device, icnv_last_error());
+    }
     for (int b = 0; b < 2; ++b) {
         dIn[b] = (double *)scratch(SLOT_SLAB_IN0 + b, sizeof(double) * slab_elems);
         if (!dIn[b]) return ICNV_E_NOMEM;
-        if (do_smooth) {
+        if (do_smooth && !mf) {
             dOut[b] = (double *)scratch(SLOT_SLAB_OUT0 + b, sizeof(double) * slab_elems);
             if (!dOut[b]) return ICNV_E_NOMEM;
         }
-        if (hmm) {
+        if (has_hmm) {
             dSt[b] = (uint8_t *)scratch(SLOT_SLAB_ST0 + b, slab_elems);
             if (!dSt[b]) return ICNV_E_NOMEM;
             if (states) {
@@ -747,10 +867,11 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         }
         if (stage_in && !(pIn[b] = (double *)pinned(b, sizeof(double) * slab_elems))) return ICNV_E_NOMEM;
         if (stage_out && do_smooth && Y && !(pOut[b] = (double *)pinned(2 + b, sizeof(double) * slab_elems))) return ICNV_E_NOMEM;
-        if (stage_out && hmm && !(pSt[b] = pinned(4 + b, st_elem * slab_elems))) return ICNV_E_NOMEM;
+        if (stage_out && has_hmm && !(pSt[b] = pinned(4 + b, st_elem * slab_elems))) return ICNV_E_NOMEM;
+        if (stage_out && mf && !(pF[b] = (double *)pinned(6 + b, sizeof(double) * slab_elems))) return ICNV_E_NOMEM;
     }
-    const int64_t n_slabs = (C + slab - 1) / slab;
-    auto slab_cells_of = [&](int64_t i) { return std::min<int64_t>(slab, C - i * slab); };
+    const int64_t n_slabs = (int64_t)s_at.size() - 1;
+    auto slab_cells_of = [&](int64_t i) { return s_at[(size_t)i + 1] - s_at[(size_t)i]; };
     // results of slab j leave the pinned ring for the caller's buffers (after its D2H has completed); together with the
     // input of slab `in` entering the ring when in >= 0 - one hand-over to the copy threads for both directions
     auto host_copies = [&](int64_t in, int64_t out) -> int {
@@ -761,13 +882,13 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
             const int b = (int)(in & 1);
             if (in >= 2) ICNV_CUDA(cudaEventSynchronize(c.ev_h2d[b]));   // the ring slot has been read by slab in-2's H2D
             d0 = pIn[b];
-            s0 = X + G * (c_lo + in * slab);
+            s0 = X + G * (c_lo + s_at[(size_t)in]);
             n0 = sizeof(double) * (size_t)G * (size_t)slab_cells_of(in);
         }
         if (out >= 0 && out < n_slabs && stage_out) {
             const int b = (int)(out & 1);
             ICNV_CUDA(cudaEventSynchronize(c.ev_d2h[b]));
-            const int64_t c0 = c_lo + out * slab, nc = slab_cells_of(out);
+            const int64_t c0 = c_lo + s_at[(size_t)out], nc = slab_cells_of(out);
             if (do_smooth && Y) {
                 d1 = Y + G * c0;
                 s1 = pOut[b];
@@ -795,7 +916,7 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     // H2D of slab i (buffer i & 1) may start once the kernels of slab i-2 have consumed the buffer
     auto issue_h2d = [&](int64_t i) -> int {
         const int b = (int)(i & 1);
-        const int64_t c0 = c_lo + i * slab, nc = slab_cells_of(i);
+        const int64_t c0 = c_lo + s_at[(size_t)i], nc = slab_cells_of(i);
         if (i >= 2) ICNV_CUDA(cudaStreamWaitEvent(sh, c.ev_comp[b], 0));
         ICNV_CUDA(cudaMemcpyAsync(dIn[b], stage_in ? pIn[b] : X + G * c0, sizeof(double) * (size_t)G * (size_t)nc,
                                   cudaMemcpyHostToDevice, sh));
@@ -803,6 +924,23 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         return ICNV_OK;
     };
     int64_t h2d_issued = 0;
+    double i3_Pi[9], i3_delta[3], i3_mean[3], i3_sd[3];
+    const HmmModel i3_hmm{3, i3_Pi, i3_delta, i3_mean, i3_sd};
+    // the median filter's local lists and events: F of unit u leaves (ev_f) before unit u+1's filter overwrites dFu
+    std::vector<int32_t> mf_off_u, mf_idx_u;
+    cudaEvent_t ev_mf = nullptr, ev_f[2] = {nullptr, nullptr};
+    struct EventsGuard {
+        cudaEvent_t *e[3];
+        ~EventsGuard() {
+            for (cudaEvent_t *p : e)
+                if (*p) cudaEventDestroy(*p);
+        }
+    } ev_guard{{&ev_mf, &ev_f[0], &ev_f[1]}};
+    if (mf) {
+        ICNV_CUDA(cudaEventCreateWithFlags(&ev_mf, cudaEventDisableTiming));
+        ICNV_CUDA(cudaEventCreateWithFlags(&ev_f[0], cudaEventDisableTiming));
+        ICNV_CUDA(cudaEventCreateWithFlags(&ev_f[1], cudaEventDisableTiming));
+    }
 
     if (do_smooth) {
         // ---- reference pre-passes on a compact copy of the reference columns (<= ~10 % of the cells) ----
@@ -813,6 +951,8 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         double *d_b = (double *)scratch(SLOT_BOUNDS, sizeof(double) * (size_t)G * 6);
         int32_t *d_iota = (int32_t *)scratch(SLOT_IDX, sizeof(int32_t) * (size_t)n_ref);
         if (!d_ref || !d_T || !d_means || !d_b || !d_iota) return ICNV_E_NOMEM;
+        if (gate && !gate->arrive(current_slot(), true))
+            return set_error(ICNV_E_NOMEM, "stopped before any output: another device could not allocate its buffers");
         for (int64_t i = 0; i < n_ref;) {  // runs of consecutive cells go up in one copy (staged: a ring slot at a time)
             int64_t j = i + 1;
             while (j < n_ref && grp_idx[j] == grp_idx[j - 1] + 1) ++j;
@@ -851,15 +991,87 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         if ((rc = icnv_dev_bounds_from_means_f64(d_means, G, n_grp, lo2, hi2, mid2, sc))) return rc;
         if (!use_bounds) lo1 = hi1 = lo2 = hi2 = nullptr;
         else mid1 = mid2 = nullptr;
+        if (i3) {
+            // .i3HMM_get_sd_trend_by_num_cells_fit (i3HMM.R:17-80): mu and sigma over every value of the reference cells after
+            // step 14.  Their final columns are a stage-D-only launch away from T (bit-identical to pass 2's: x - 0.0 == x); the
+            // per-cell (sum, sd) pairs are combined in list order, exactly as icnv_mean_sd_f64 forms them.  T then holds the pairs.
+            rc = icnv_dev_cell_pipeline_f64(d_T, G, G, nullptr, n_ref, d_ref, G, chr_start, chr_len, K, 0, nullptr, nullptr,
+                                            nullptr, 0.0, 0, 0, lo2, hi2, mid2, 1, d_flag, sc);
+            if (rc) return rc;
+            if ((rc = icnv_dev_column_stats_f64(d_ref, G, d_iota, n_ref, d_T, d_T + n_ref, sc))) return rc;
+            std::vector<double> h(2 * (size_t)n_ref);
+            ICNV_CUDA(cudaMemcpyAsync(h.data(), d_T, sizeof(double) * 2 * (size_t)n_ref, cudaMemcpyDeviceToHost, sc));
+            ICNV_CUDA(cudaStreamSynchronize(sc));
+            double mu, sigma;
+            icnv_combine_cell_stats(h.data(), h.data() + n_ref, n_ref, G, &mu, &sigma);
+            // .i3HMM_get_HMM (i3HMM.R:99-156) with use_KS = FALSE: states at mu -+ |qnorm(p, 0, sigma)|, sd sigma, transition
+            // diagonal 1 - 5t as the reference writes it
+            const double d = std::fabs(qnorm_as241(i3->p_val, 0.0, sigma));
+            for (int k = 0; k < 9; ++k) i3_Pi[k] = (k % 4 == 0) ? 1 - 5 * i3->t : i3->t;
+            i3_delta[0] = i3_delta[2] = i3->t;
+            i3_delta[1] = 1 - 5 * i3->t;
+            i3_mean[0] = mu - d; i3_mean[1] = mu; i3_mean[2] = mu + d;
+            i3_sd[0] = i3_sd[1] = i3_sd[2] = sigma;
+            if (i3->model) {
+                i3->model[0] = mu;
+                i3->model[1] = sigma;
+                i3->model[2] = d;
+            }
+            hmm = &i3_hmm;
+        }
     }
+
+    // apply_median_filtering on the unit that slab i closes: the lists inside it with unit-local indices, K4 on the unit's Y,
+    // then F down - straight into the caller's matrix, or through two pinned chunks while the copy threads empty the other
+    auto unit_median_filter = [&](int64_t i) -> int {
+        const int64_t u0 = unit_lo[(size_t)i], nu = s_at[(size_t)i + 1] - u0;
+        mf_off_u.assign(1, 0);
+        mf_idx_u.clear();
+        for (int k = 0; k < i3->n_mf; ++k) {
+            const int32_t a = i3->mf_off[k], e = i3->mf_off[k + 1];
+            if (i3->mf_idx[a] < c_lo + u0 || i3->mf_idx[a] >= c_lo + u0 + nu) continue;   // a list lies inside one unit
+            for (int32_t q = a; q < e; ++q) mf_idx_u.push_back((int32_t)(i3->mf_idx[q] - (c_lo + u0)));
+            mf_off_u.push_back((int32_t)mf_idx_u.size());
+        }
+        ICNV_CUDA(cudaStreamWaitEvent(sc, ev_f[0], 0));   // (a recorded-never event is complete)
+        int rc2 = icnv_dev_median_filter_f64(dYu, dFu, G, nu, chr_start, chr_len, K, mf_off_u.data(), mf_idx_u.data(),
+                                             (int)mf_off_u.size() - 1, i3->mf_window, sc);
+        if (rc2) return rc2;
+        ICNV_CUDA(cudaEventRecord(ev_mf, sc));
+        ICNV_CUDA(cudaStreamWaitEvent(sd, ev_mf, 0));
+        double *F0 = i3->F + G * (c_lo + u0);
+        if (!stage_out) {
+            ICNV_CUDA(cudaMemcpyAsync(F0, dFu, sizeof(double) * (size_t)G * (size_t)nu, cudaMemcpyDeviceToHost, sd));
+            ICNV_CUDA(cudaEventRecord(ev_f[0], sd));
+            return ICNV_OK;
+        }
+        const int64_t n_chunks = (nu + slab - 1) / slab;
+        auto chunk_bytes = [&](int64_t k) { return sizeof(double) * (size_t)G * (size_t)std::min<int64_t>(slab, nu - k * slab); };
+        for (int64_t k = 0; k <= n_chunks; ++k) {
+            if (k < n_chunks) {   // pF[k & 1] was emptied by the copy of chunk k-2, one trip ago
+                ICNV_CUDA(cudaMemcpyAsync(pF[k & 1], dFu + G * slab * k, chunk_bytes(k), cudaMemcpyDeviceToHost, sd));
+                ICNV_CUDA(cudaEventRecord(ev_f[k & 1], sd));
+            }
+            if (k >= 1) {
+                ICNV_CUDA(cudaEventSynchronize(ev_f[(k - 1) & 1]));
+                pool->copy2(F0 + G * slab * (k - 1), pF[(k - 1) & 1], chunk_bytes(k - 1), nullptr, nullptr, 0);
+            }
+        }
+        ICNV_CUDA(cudaEventRecord(ev_f[0], sd));
+        return ICNV_OK;
+    };
 
     if (stage_in) {   // the first slab enters the ring while the reference pre-passes run on the device
         if ((rc = host_copies(0, -1))) return rc;
     }
     for (int64_t i = 0; i < n_slabs; ++i) {
         const int b = (int)(i & 1);
-        const int64_t c0 = c_lo + i * slab, nc = slab_cells_of(i);
+        const int64_t c0 = c_lo + s_at[(size_t)i], nc = slab_cells_of(i);
         const size_t bytes = sizeof(double) * (size_t)G * (size_t)nc;
+        // the unit buffer: slab i writes its own columns of it; the first slab of a unit also overwrites what the previous
+        // unit's last slab (i-1) has to have left through D2H
+        double *d_out = mf ? dYu + G * (s_at[(size_t)i] - unit_lo[(size_t)i]) : dOut[b];
+        if (mf && i >= 1 && unit_lo[(size_t)i] != unit_lo[(size_t)i - 1]) ICNV_CUDA(cudaStreamWaitEvent(sc, c.ev_d2h[b ^ 1], 0));
         if (stage_in) {
             if (h2d_issued <= i && (rc = issue_h2d(h2d_issued++))) return rc;
         } else {
@@ -871,10 +1083,10 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         if (i >= 2) ICNV_CUDA(cudaStreamWaitEvent(sc, c.ev_d2h[b], 0));
         const double *hmm_in = dIn[b];
         if (do_smooth) {
-            rc = icnv_dev_cell_pipeline_f64(dIn[b], G, G, nullptr, nc, dOut[b], G, chr_start, chr_len, K, apply_log, lo1, hi1,
+            rc = icnv_dev_cell_pipeline_f64(dIn[b], G, G, nullptr, nc, d_out, G, chr_start, chr_len, K, apply_log, lo1, hi1,
                                             mid1, threshold, window, 1, lo2, hi2, mid2, 1, d_flag, sc);
             if (rc) return rc;
-            hmm_in = dOut[b];
+            hmm_in = d_out;
         }
         if (hmm) {
             rc = icnv_dev_viterbi_f64(hmm_in, G, nc, chr_start, chr_len, K, hmm->m, hmm->Pi, hmm->delta, hmm->mean, hmm->sd,
@@ -885,7 +1097,7 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         ICNV_CUDA(cudaEventRecord(c.ev_comp[b], sc));
         // D2H (staged: the ring slot of slab i-2 was emptied by host_copies(.., i-2) below, two iterations ago)
         ICNV_CUDA(cudaStreamWaitEvent(sd, c.ev_comp[b], 0));
-        if (do_smooth && Y) ICNV_CUDA(cudaMemcpyAsync(stage_out ? pOut[b] : Y + G * c0, dOut[b], bytes, cudaMemcpyDeviceToHost, sd));
+        if (do_smooth && Y) ICNV_CUDA(cudaMemcpyAsync(stage_out ? pOut[b] : Y + G * c0, d_out, bytes, cudaMemcpyDeviceToHost, sd));
         if (hmm && states)
             ICNV_CUDA(cudaMemcpyAsync(stage_out ? (int32_t *)pSt[b] : states + G * c0, dW[b],
                                       sizeof(int32_t) * (size_t)G * (size_t)nc, cudaMemcpyDeviceToHost, sd));
@@ -893,6 +1105,7 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
             ICNV_CUDA(cudaMemcpyAsync(stage_out ? (uint8_t *)pSt[b] : states8 + G * c0, dSt[b], (size_t)G * (size_t)nc,
                                       cudaMemcpyDeviceToHost, sd));
         ICNV_CUDA(cudaEventRecord(c.ev_d2h[b], sd));
+        if (mf && unit_end[(size_t)i] && (rc = unit_median_filter(i))) return rc;
         // host side of the ring while the device works on slab i: slab i+1 in, slab i-1 out
         if (stage_in || stage_out)
             if ((rc = host_copies(stage_in ? i + 1 : -1, stage_out ? i - 1 : -1))) return rc;
@@ -908,21 +1121,41 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
 static int host_pipeline(Ctx &c0, const double *X, double *Y, int32_t *states, uint8_t *states8, int64_t G, int64_t C,
                          const int32_t *chr_start, const int32_t *chr_len, int K, int do_smooth, const int32_t *grp_off,
                          const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window, int use_bounds,
-                         const HmmModel *hmm) {
+                         const HmmModel *hmm, const I3Fused *i3 = nullptr) {
     const int n_dev = (int)std::min<int64_t>(std::max(1, device_slots()), std::max<int64_t>(1, C / 64));
-    const bool pageable = !is_pinned(X) || (Y && !is_pinned(Y)) || (states && !is_pinned(states)) || (states8 && !is_pinned(states8));
+    const bool pageable = !is_pinned(X) || (Y && !is_pinned(Y)) || (states && !is_pinned(states)) || (states8 && !is_pinned(states8)) ||
+                          (i3 && i3->F && !is_pinned(i3->F));
     const int nt = pool_threads_per_device();
     if (n_dev <= 1) {
         std::unique_ptr<CopyPool> pool(pageable ? new CopyPool(nt) : nullptr);
         return host_pipeline_range(c0, X, Y, states, states8, G, 0, C, chr_start, chr_len, K, do_smooth, grp_off, grp_idx, n_grp,
-                                   apply_log, threshold, window, use_bounds, hmm, pool.get());
+                                   apply_log, threshold, window, use_bounds, hmm, pool.get(), i3);
+    }
+    // even shares; with the median filter each cut moves to the nearest column no list's span crosses
+    std::vector<int64_t> cut((size_t)n_dev + 1);
+    for (int d = 0; d <= n_dev; ++d) {
+        cut[(size_t)d] = C * d / n_dev;
+        if (i3 && i3->F) cut[(size_t)d] = std::max(d ? cut[(size_t)d - 1] : 0, i3->cut_near(cut[(size_t)d]));
+    }
+    int reporter = 0;   // the first device with cells reports the i3 model (every device computes the same bits)
+    while (reporter < n_dev - 1 && cut[(size_t)reporter] == cut[(size_t)reporter + 1]) ++reporter;
+    std::vector<I3Fused> i3d;
+    if (i3) {
+        i3d.assign((size_t)n_dev, *i3);
+        for (int d = 0; d < n_dev; ++d)
+            if (d != reporter) i3d[(size_t)d].model = nullptr;
     }
     std::vector<int> rcs((size_t)n_dev, ICNV_OK);
     std::vector<std::string> msgs((size_t)n_dev);
     std::vector<std::thread> th;
     const int caller_slot = current_slot();
+    int n_busy = 0;
+    for (int d = 0; d < n_dev; ++d) n_busy += cut[(size_t)d] < cut[(size_t)d + 1];
+    // the fused i3 call promises that a unit that does not fit is refused before any output is written
+    std::unique_ptr<StartGate> gate(i3 && i3->F ? new StartGate(n_dev, n_busy) : nullptr);
     for (int d = 0; d < n_dev; ++d) {
-        const int64_t lo = C * d / n_dev, hi = C * (d + 1) / n_dev;
+        const int64_t lo = cut[(size_t)d], hi = cut[(size_t)d + 1];
+        if (lo == hi) continue;
         th.emplace_back([&, d, lo, hi] {
             set_current_slot(d);
             Ctx &c = ctx();
@@ -933,14 +1166,20 @@ static int host_pipeline(Ctx &c0, const double *X, double *Y, int32_t *states, u
             if (!rc) {
                 std::unique_ptr<CopyPool> pool(pageable ? new CopyPool(nt) : nullptr);
                 rc = host_pipeline_range(c, X, Y, states, states8, G, lo, hi, chr_start, chr_len, K, do_smooth, grp_off, grp_idx,
-                                         n_grp, apply_log, threshold, window, use_bounds, hmm, pool.get());
+                                         n_grp, apply_log, threshold, window, use_bounds, hmm, pool.get(),
+                                         i3 ? &i3d[(size_t)d] : nullptr, gate.get());
             }
+            if (gate) gate->arrive(d, rc == ICNV_OK);   // a range that failed before the gate still has to open it
             rcs[(size_t)d] = rc;
             if (rc) msgs[(size_t)d] = icnv_last_error();   // the message is per thread: carry it to the caller
         });
     }
     for (auto &t : th) t.join();
     cudaSetDevice(c0.device);
+    if (gate && gate->first_fail >= 0) {   // report the device that could not start, not the ones it stopped
+        const int d = gate->first_fail;
+        return set_error(rcs[(size_t)d], "device %d: %s", ctx_of(d).device, msgs[(size_t)d].c_str());
+    }
     for (int d = 0; d < n_dev; ++d)
         if (rcs[(size_t)d]) return set_error(rcs[(size_t)d], "device %d: %s", ctx_of(d).device, msgs[(size_t)d].c_str());
     return ICNV_OK;
@@ -991,6 +1230,44 @@ int icnv_smooth_hmm_u8_f64(const double *X, double *Y, uint8_t *states, int64_t 
                            const double *delta, const double *mean, const double *sd) {
     return smooth_hmm_impl(X, Y, nullptr, states, G, C, chr_start, chr_len, K, grp_off, grp_idx, n_grp, apply_log, threshold,
                            window, use_bounds, m, Pi, delta, mean, sd);
+}
+
+/* Fused i3 pass (see the header): smooth block, the i3 model of its reference cells, per-cell i3 HMM and
+ * apply_median_filtering over the lists mf_*, one read of X and one write of each output. */
+int icnv_smooth_i3_hmm_u8_f64(const double *X, double *Y, uint8_t *states, double *F, int64_t G, int64_t C,
+                              const int32_t *chr_start, const int32_t *chr_len, int K, const int32_t *grp_off,
+                              const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window, int use_bounds,
+                              double i3_p_val, double t, const int32_t *mf_off, const int32_t *mf_idx, int n_mf,
+                              int mf_window, double *model) {
+    ICNV_HOST_PROLOGUE();
+    if (!X || !Y || !states || !model || G <= 1 || C <= 0)
+        return set_error(ICNV_E_BAD_ARG, "icnv_smooth_i3_hmm_u8_f64: bad argument");
+    if (!(i3_p_val > 0.0 && i3_p_val < 1.0)) return set_error(ICNV_E_BAD_ARG, "i3_p_val must lie in (0, 1)");
+    if (window >= 2 && (window & 1) == 0)
+        return set_error(ICNV_E_BAD_ARG, "window_length %d is even: the reference's behaviour is accidental there", window);
+    int rc = validate_chr(G, chr_start, chr_len, K);
+    if (rc) return rc;
+    if ((rc = validate_groups(C, grp_off, grp_idx, n_grp, false))) return rc;
+    I3Fused i3{i3_p_val, t, model, nullptr, mf_off, mf_idx, n_mf, mf_window, {}};
+    if (F) {   // no lists: every cell is in none, so F is a copy of Y, as icnv_median_filter_f64 makes it
+        if (mf_window < 3 || (mf_window & 1) == 0)
+            return set_error(ICNV_E_BAD_ARG, "window_size must be an odd number >= 3 (noise_reduction.R:48-50)");
+        if (n_mf < 0) return set_error(ICNV_E_BAD_ARG, "n_mf < 0");
+        if (n_mf > 0 && (rc = validate_groups(C, mf_off, mf_idx, n_mf, false))) return rc;
+        std::vector<std::pair<int64_t, int64_t>> sp((size_t)n_mf);
+        for (int k = 0; k < n_mf; ++k) {
+            const auto mm = std::minmax_element(mf_idx + mf_off[k], mf_idx + mf_off[k + 1]);
+            sp[(size_t)k] = {*mm.first, (int64_t)*mm.second + 1};
+        }
+        std::sort(sp.begin(), sp.end());
+        for (const auto &v : sp) {
+            if (!i3.spans.empty() && v.first < i3.spans.back().second) i3.spans.back().second = std::max(i3.spans.back().second, v.second);
+            else i3.spans.push_back(v);
+        }
+        i3.F = F;
+    }
+    return host_pipeline(c, X, Y, nullptr, states, G, C, chr_start, chr_len, K, 1, grp_off, grp_idx, n_grp, apply_log, threshold,
+                         window, use_bounds, nullptr, &i3);
 }
 
 static int viterbi_impl(const double *X, int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len, int K,

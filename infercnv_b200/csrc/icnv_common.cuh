@@ -75,9 +75,10 @@ struct Ctx {
     // nothing from pageable host memory (such a copy may synchronise the host with the stream)
     std::vector<unsigned char> up_segs, up_items;
     cudaStream_t up_segs_stream = nullptr, up_items_stream = nullptr;   // an upload orders only the stream it was issued on
-    // pinned staging ring of the host-pointer entry points (pageable caller memory, e.g. an R matrix): two slabs in, two out
-    void *pin_ptr[6] = {};
-    size_t pin_bytes[6] = {};
+    // pinned staging ring of the host-pointer entry points (pageable caller memory, e.g. an R matrix): two slabs in, two out,
+    // two for the states and two for the median-filtered chunks of the fused i3 call
+    void *pin_ptr[8] = {};
+    size_t pin_bytes[8] = {};
     // tuning switches, read from the environment ONCE in icnv_init (never at launch time); -1 / 0 = library default
     int opt_cell_kernel = 0, opt_cell_nt = 0, opt_cell_variant = -1, opt_cell_padq = 1, opt_cell_lfix = 1;
     long opt_slab_cells = 0;

@@ -400,19 +400,63 @@ b200_get_predicted_CNV_regions <- function(infercnv_obj, by=c("consensus", "subc
 ## (R/inferCNV_ops.R:771, 865, 911, 952, 1031), so this is for callers that drive the steps themselves, or for a maintainer's
 ## three-line change in run() (INTEGRATION.md, "fused block").  Input: the object after step 3 (depth-normalised counts, before
 ## log2) when apply_log = TRUE, after step 4 otherwise; use_bounds / max_centered_threshold / window_length as in run().
-## HMM_info (optional): the list .get_HMM() / .i3HMM_get_HMM() returns -> per-cell states are predicted on the block's output
-## in the same pass.  Returns list(infercnv_obj = <after step 14>, hmm_obj = <states object or NULL>); NULL when the input is
-## outside the GPU path's envelope (the caller then runs the R steps).
+## HMM_info (optional): the list .get_HMM() returns (i6, a fixed model) -> per-cell states are predicted on the block's output
+## in the same pass.  An i3 model cannot be passed in: .i3HMM_get_HMM() is built from this block's own output (mu and sigma
+## of the reference cells after step 14).  For i3 leave HMM_info NULL and set i3_p_val (t and use_KS as in run()): the
+## library fixes the model from the reference cells inside the pass.  median_filter_window (optional, i3 path): also
+## apply_median_filtering(window_size = median_filter_window) on the block's output, over the lists
+## b200_apply_median_filtering builds from THIS object: its tumor_subclusters and its reference groups.  run() defines
+## tumor_subclusters only at step 15, after the block, so on an object straight from step 3 they are absent and the
+## observation cells come back unfiltered (copied, as apply_median_filtering itself leaves them on that object); a caller
+## who wants run()'s step-22 result sets tumor_subclusters first (with partition_method = "none": one subcluster per
+## observation group).  use_KS = TRUE needs R's KS delta before the HMM: NULL is returned.
+## Returns list(infercnv_obj = <after step 14>, hmm_obj = <states object or NULL>), on the i3 path also median_obj (the
+## median-filtered object or NULL) and sd_trend (.i3HMM_get_sd_trend_by_num_cells_fit's list); NULL when the input is outside
+## the GPU path's envelope (the caller then runs the R steps).
 infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_centered_threshold=3, use_bounds=TRUE,
-                                          apply_log=TRUE, HMM_info=NULL) {
+                                          apply_log=TRUE, HMM_info=NULL, i3_p_val=NULL, t=1e-6, use_KS=FALSE,
+                                          median_filter_window=NULL) {
     m <- infercnv_obj@expr.data
     codes <- .icnv_chr_codes(infercnv_obj)
+    i3 <- is.null(HMM_info) && !is.null(i3_p_val)
     if (!.icnv_enabled() || !.icnv_ok(m) || is.null(codes) || window_length < 2 || window_length %% 2 == 0 ||
         is.na(max_centered_threshold) || !is.numeric(max_centered_threshold)) return(NULL)
-    futile.logger::flog.info(sprintf("::smooth block (steps 4, 8-12, 14%s) in one pass (GPU)", if (is.null(HMM_info)) "" else " + per-cell HMM"))
+    if (i3 && (isTRUE(use_KS) || !is.numeric(i3_p_val) || !(i3_p_val > 0 && i3_p_val < 1) ||
+               (!is.null(median_filter_window) && (median_filter_window %% 2 != 1 || median_filter_window < 3)))) return(NULL)
+    futile.logger::flog.info(sprintf("::smooth block (steps 4, 8-12, 14%s) in one pass (GPU)",
+                                     if (i3) paste0(" + i3 model + per-cell HMM", if (is.null(median_filter_window)) "" else " + median filter")
+                                     else if (is.null(HMM_info)) "" else " + per-cell HMM"))
     refs <- .icnv_ref_groups(infercnv_obj)
     hmm_obj <- NULL
-    if (is.null(HMM_info)) {
+    median_obj <- NULL
+    sd_trend <- NULL
+    if (i3) {
+        lists <- NULL
+        if (!is.null(median_filter_window)) {   # as b200_apply_median_filtering builds them
+            lists <- list()
+            for (tt in names(infercnv_obj@observation_grouped_cell_indices))
+                lists <- c(lists, lapply(infercnv_obj@tumor_subclusters[["subclusters"]][[tt]], as.integer))
+            lists <- c(lists, lapply(infercnv_obj@reference_grouped_cell_indices, as.integer))
+        }
+        res <- .icnv_try(.Call("icnvR_smooth_i3_hmm", m, codes, refs, isTRUE(apply_log), as.double(max_centered_threshold),
+                               as.integer(window_length), isTRUE(use_bounds), as.double(i3_p_val), as.double(t), lists,
+                               as.integer(if (is.null(median_filter_window)) 7L else median_filter_window)), "smooth_i3_hmm")
+        if (is.null(res)) return(NULL)
+        infercnv_obj@expr.data <- .icnv_keep_names(res[[1]], m)
+        hmm_obj <- infercnv_obj
+        hmm_obj@expr.data <- .icnv_keep_names(res[[2]], m)
+        if (!is.null(res[[3]])) {
+            median_obj <- infercnv_obj
+            median_obj@expr.data <- .icnv_keep_names(res[[3]], m)
+        }
+        mu <- res[[4]][1]; sigma <- res[[4]][2]; mean_delta <- res[[4]][3]
+        message("mean_delta: ", mean_delta, ", at sigma: ", sigma, ", and pval: ", i3_p_val)
+        ## the reference draws the KS delta even with use_KS = FALSE (rnorm + ks.test, i3HMM.R:68); drawing it here keeps R's
+        ## random stream where every later RNG-dependent step expects it
+        KS_delta <- infercnv:::get_HoneyBADGER_setGexpDev(gexp.sd=sigma, alpha=i3_p_val, k_cells=length(unlist(refs)))
+        message("KS_delta: ", KS_delta, ", at sigma: ", sigma, ", and pval: ", i3_p_val)
+        sd_trend <- list(mu=mu, sigma=sigma, mean_delta=mean_delta, KS_delta=KS_delta)
+    } else if (is.null(HMM_info)) {
         res <- .icnv_try(.Call("icnvR_smooth_block", m, codes, refs, isTRUE(apply_log), as.double(max_centered_threshold),
                                as.integer(window_length), isTRUE(use_bounds)), "smooth_block")
         if (is.null(res)) return(NULL)
@@ -433,6 +477,7 @@ infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_c
         if (is.null(h)) return(NULL)
         infercnv_obj@.hspike <- h$infercnv_obj
     }
+    if (i3) return(list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj, median_obj = median_obj, sd_trend = sd_trend))
     list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj)
 }
 

@@ -155,6 +155,44 @@ SEXP icnvR_smooth_hmm(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_log
     return ans;
 }
 
+/* the i3 counterpart (icnv_smooth_i3_hmm_u8_f64): run() steps 4, 8-12, 14, the i3 model of the reference cells, step 17 per
+ * cell and, with median_lists non-NULL, apply_median_filtering (noise_reduction.R:43-113) in one pass.
+ * Returns list(expr, states, median_filtered or NULL, c(mu, sigma, mean_delta)). */
+SEXP icnvR_smooth_i3_hmm(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_log, SEXP threshold, SEXP window_length,
+                         SEXP use_bounds, SEXP i3_p_val, SEXP t, SEXP median_lists, SEXP median_window) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int32_t *cs = NULL, *cl = NULL, *off = NULL, *idx = NULL, *moff = NULL, *midx = NULL;
+    int K = chr_to_ranges(chr_codes, &cs, &cl);
+    int n_grp = list_to_csr(ref_groups, &off, &idx);
+    const int filter = !Rf_isNull(median_lists);
+    int n_mf = filter ? list_to_csr(median_lists, &moff, &midx) : 0;
+    uint8_t *st = (uint8_t *)malloc((size_t)(G * C));
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, 4));
+    SEXP y = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    SEXP states = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    SEXP f = PROTECT(filter ? Rf_allocMatrix(REALSXP, (int)G, (int)C) : R_NilValue);
+    SEXP model = PROTECT(Rf_allocVector(REALSXP, 3));
+    int rc = (K < 0 || n_grp < 0 || n_mf < 0 || !st)
+                 ? ICNV_E_NOMEM
+                 : icnv_smooth_i3_hmm_u8_f64(REAL(expr), REAL(y), st, filter ? REAL(f) : NULL, G, C, cs, cl, K, off, idx, n_grp,
+                                             Rf_asLogical(apply_log), Rf_asReal(threshold), Rf_asInteger(window_length),
+                                             Rf_asLogical(use_bounds), Rf_asReal(i3_p_val), Rf_asReal(t), moff, midx, n_mf,
+                                             filter ? Rf_asInteger(median_window) : 0, REAL(model));
+    if (rc == 0) {
+        double *out = REAL(states);   /* the reference keeps states as doubles (i3HMM.R:222) */
+        for (int64_t i = 0; i < G * C; ++i) out[i] = (st[i] == 255) ? -1.0 : (double)st[i];
+    }
+    SET_VECTOR_ELT(ans, 0, y);
+    SET_VECTOR_ELT(ans, 1, states);
+    SET_VECTOR_ELT(ans, 2, f);
+    SET_VECTOR_ELT(ans, 3, model);
+    free(cs); free(cl); free(off); free(idx); free(moff); free(midx); free(st);
+    UNPROTECT(5);
+    fail_if(rc);
+    return ans;
+}
+
 /* icnv_init_devices: single-process multi-GPU (infercnv::run() is one R process).  ids = NULL: every GPU present. */
 SEXP icnvR_init_devices(SEXP ids) {
     int rc = Rf_isNull(ids) ? icnv_init_devices(0, NULL) : icnv_init_devices(Rf_length(ids), INTEGER(ids));
@@ -755,6 +793,7 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_viterbi_per_chr", (DL_FUNC)&icnvR_viterbi_per_chr, 9}, {"icnvR_scale", (DL_FUNC)&icnvR_scale, 1},
     {"icnvR_clear_noise_threshold", (DL_FUNC)&icnvR_clear_noise_threshold, 4},
     {"icnvR_smooth_hmm", (DL_FUNC)&icnvR_smooth_hmm, 11},   {"icnvR_init_devices", (DL_FUNC)&icnvR_init_devices, 1},
+    {"icnvR_smooth_i3_hmm", (DL_FUNC)&icnvR_smooth_i3_hmm, 11},
     {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1}, {"icnvR_hclust", (DL_FUNC)&icnvR_hclust, 2},
     {"icnvR_knn", (DL_FUNC)&icnvR_knn, 2},
     {"icnvR_runmean", (DL_FUNC)&icnvR_runmean, 4},

@@ -225,6 +225,38 @@ def smooth_block(infercnv_obj: Infercnv, window_length: int = 101, max_centered_
     return obj
 
 
+def smooth_block_i3_hmm(infercnv_obj: Infercnv, window_length: int = 101, max_centered_threshold: float = 3.0,
+                        apply_log: bool = True, use_bounds: bool = True, i3_p_val: float = 0.05, t: float = 1e-6,
+                        median_filter_window: Optional[int] = None):
+    """The i3 counterpart of smooth_block: run() steps 4, 8-12, 14, .i3HMM_get_sd_trend_by_num_cells_fit on the block's
+    reference cells, the per-cell i3 HMM (i3HMM.R:180-225, use_KS = FALSE) and, with median_filter_window, the
+    apply_median_filtering of that window (noise_reduction.R:43-113, the lists of apply_median_filtering below) - one library
+    call.  Returns (obj after step 14, states object, median-filtered object or None, sd_trend); sd_trend's KS_delta is None
+    (it comes from R's RNG)."""
+    obj = copy.copy(infercnv_obj)
+    cs, cl = obj.chr_ranges()
+    lists = None
+    if median_filter_window is not None:   # without tumor_subclusters (run() sets them at step 15) only references are listed
+        subs = (obj.tumor_subclusters or {}).get("subclusters", {})
+        lists = [np.asarray(idx) for tt in obj.observation_grouped_cell_indices for idx in subs.get(tt, {}).values()]
+        lists += [np.asarray(idx) for idx in obj.reference_grouped_cell_indices.values()]
+    Y, S, F, model = api.smooth_i3_hmm(obj.expr_data, cs, cl, _ref_groups(obj), i3_p_val=i3_p_val, t=t, median_lists=lists,
+                                       median_window=median_filter_window or 7, apply_log=apply_log,
+                                       threshold=max_centered_threshold, window_length=window_length, use_bounds=use_bounds)
+    obj.expr_data = Y
+    hmm_obj = copy.copy(obj)
+    st = S.astype(np.float64)
+    st[S == 255] = -1.0
+    hmm_obj.expr_data = np.asfortranarray(st)
+    med_obj = None
+    if F is not None:
+        med_obj = copy.copy(obj)
+        med_obj.expr_data = F
+    if obj.hspike is not None:
+        obj.hspike = smooth_block(obj.hspike, window_length, max_centered_threshold, apply_log, use_bounds)
+    return obj, hmm_obj, med_obj, dict(model, KS_delta=None)
+
+
 def apply_median_filtering(infercnv_obj: Infercnv, window_size: int = 7, on_observations: bool = True,
                            on_references: bool = True) -> Infercnv:
     """R/noise_reduction.R:43-89.  Observations are filtered per tumour subcluster, references per
