@@ -210,6 +210,39 @@ ICNV_API int icnv_smooth_i3_hmm_u8_f64(const double *X, double *Y, uint8_t *stat
                                        int use_bounds, double i3_p_val, double t, const int32_t *mf_off,
                                        const int32_t *mf_idx, int n_mf, int mf_window, double *model);
 
+/* Group-mode twins of the two fused calls: run() steps 4..14 and step 17 for analysis_mode = "samples" and "subclusters"
+ * (tumor_subcluster_partition_method = "random_trees", whose partition is made before the block), prune_outliers = FALSE.
+ * The HMM runs on the group means of Y over the lists hmm_off / hmm_idx (CSR, n_hmm groups), as icnv_viterbi_u8_f64
+ * with those lists does.
+ *   Y       = icnv_smooth_block_f64 with the same arguments (bit-identical).
+ *   states  = icnv_viterbi_u8_f64(Y, hmm lists, m, Pi, delta, mean, sd) (bit-identical): sd[m * n_hmm] holds every
+ *             group's state sds and each group's trace uses their median.  A cell in no list gets 255; a cell in several
+ *             lists gets the trace of the last one (R's <<- overwrite does the same).
+ *   i3:       model = {mu, sigma, mean_delta} exactly as icnv_smooth_i3_hmm_u8_f64 returns it; states = the same group
+ *             Viterbi under .i3HMM_get_HMM(model) with sd sigma for every group.  No median filter: callers run
+ *             icnv_median_filter_f64 on Y.
+ * The cells stream through the device in list order (every list entry, then the cells in no list), so a group's means are
+ * summed in dev_group_means' fixed 32-entry chunks; the device holds the slabs, G x n_hmm means and traces, and the sums of
+ * the group open at a slab boundary - never the matrix.  Page-locked X and Y are copied one run of consecutive columns at a
+ * time; pageable ones are gathered into and scattered from the pinned ring by the copy threads.
+ * Several devices (icnv_init_devices): the list order is cut at the group boundaries nearest to even shares, each group's
+ * means and trace are computed on one device, and every device reduces all reference cells itself, so every output is
+ * independent of the device count and of ICNV_SLAB_CELLS.
+ * BAD_ARG (nothing written): n_hmm == 0 (the per-cell calls cover it), an empty group, an index out of range, a
+ * non-positive median sd; for i3 also an even window, i3_p_val outside (0, 1), G < 2.  Buffers that do not fit are
+ * ICNV_E_NOMEM before any output is written, on every device. */
+ICNV_API int icnv_smooth_hmm_groups_u8_f64(const double *X, double *Y, uint8_t *states, int64_t G, int64_t C,
+                                           const int32_t *chr_start, const int32_t *chr_len, int K, const int32_t *grp_off,
+                                           const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window,
+                                           int use_bounds, const int32_t *hmm_off, const int32_t *hmm_idx, int n_hmm, int m,
+                                           const double *Pi, const double *delta, const double *mean, const double *sd);
+ICNV_API int icnv_smooth_i3_hmm_groups_u8_f64(const double *X, double *Y, uint8_t *states, int64_t G, int64_t C,
+                                              const int32_t *chr_start, const int32_t *chr_len, int K,
+                                              const int32_t *grp_off, const int32_t *grp_idx, int n_grp, int apply_log,
+                                              double threshold, int window, int use_bounds, const int32_t *hmm_off,
+                                              const int32_t *hmm_idx, int n_hmm, double i3_p_val, double t,
+                                              double *model);
+
 /* Viterbi.dthmm.adj, R/inferCNV_HMM.R:1101-1176, batched over the drivers
  * predict_CNV_via_HMM_on_indiv_cells (HMM.R:284-324), ..._on_tumor_subclusters (:345-408),
  * ..._on_whole_tumor_samples (:509-567) and the i3 twins (R/inferCNV_i3HMM.R:180-389).

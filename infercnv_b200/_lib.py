@@ -47,6 +47,10 @@ SIGNATURES = {
                                        c_int, c_int, _P, _P, _P, _P]),
     "icnv_smooth_i3_hmm_u8_f64": (c_int, [_P, _P, _P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,
                                           c_int, c_int, ct.c_double, ct.c_double, _P, _P, c_int, c_int, _P]),
+    "icnv_smooth_hmm_groups_u8_f64": (c_int, [_P, _P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,
+                                              c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P]),
+    "icnv_smooth_i3_hmm_groups_u8_f64": (c_int, [_P, _P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, ct.c_double,
+                                                 c_int, c_int, _P, _P, c_int, ct.c_double, ct.c_double, _P]),
     "icnv_viterbi_f64": (c_int, [_P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "icnv_viterbi_u8_f64": (c_int, [_P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "icnv_median_filter_f64": (c_int, [_P, _P, c_i64, c_i64, _P, _P, c_int, _P, _P, c_int, c_int]),

@@ -199,9 +199,12 @@ def smooth_block(X, chr_start, chr_len, ref_groups, apply_log=True, threshold=3.
 
 
 def smooth_hmm(X, chr_start, chr_len, ref_groups, Pi, delta, mean, sd, apply_log=True, threshold=3.0, window_length=101,
-               use_bounds=True, out=None, out_states=None):
+               use_bounds=True, out=None, out_states=None, groups=None):
     """Fused smooth block + per-cell HMM (one upload of the matrix).  Returns (Y, states).  States come back as int32
-    by default; pass a uint8 `out_states` for the one-byte wire format (icnv_smooth_hmm_u8_f64)."""
+    by default; pass a uint8 `out_states` for the one-byte wire format (icnv_smooth_hmm_u8_f64).
+
+    groups: the HMM lists of analysis_mode "samples" / "subclusters" (icnv_smooth_hmm_groups_u8_f64): states are the group
+    Viterbi's, uint8 with 255 for cells in no group, and sd holds m entries per group (or m, shared)."""
     X = _f64(X)
     G, C = X.shape
     cs, cl = _i32(chr_start), _i32(chr_len)
@@ -209,6 +212,21 @@ def smooth_hmm(X, chr_start, chr_len, ref_groups, Pi, delta, mean, sd, apply_log
     Pi = np.asfortranarray(Pi, dtype=np.float64)
     delta, mean, sd = (np.ascontiguousarray(v, dtype=np.float64) for v in (delta, mean, sd))
     Y = np.empty_like(X, order="F") if out is None else out
+    if groups is not None:
+        m, ng = Pi.shape[0], len(groups)
+        if sd.size == m:
+            sd = np.tile(sd, ng)
+        if sd.size != m * ng:
+            raise ValueError("sd must have m entries per group")
+        S = np.empty((G, C), dtype=np.uint8, order="F") if out_states is None else out_states
+        if S.dtype != np.uint8 or S.shape != (G, C) or not S.flags.f_contiguous:
+            raise ValueError("with groups, out_states must be a Fortran-ordered (G, C) uint8 array")
+        hoff, hidx = groups_to_csr(groups)
+        _lib.check(_lib.load().icnv_smooth_hmm_groups_u8_f64(
+            _p(X), _p(Y), _p(S), G, C, _p(cs), _p(cl), len(cs), _p(off), _p(idx), len(ref_groups), int(bool(apply_log)),
+            float(threshold), int(window_length), int(bool(use_bounds)), _p(hoff), _p(hidx), ng, m, _p(Pi), _p(delta),
+            _p(mean), _p(sd)))
+        return Y, S
     S = np.empty((G, C), dtype=np.int32, order="F") if out_states is None else out_states
     if S.dtype not in (np.int32, np.uint8) or S.shape != (G, C) or not S.flags.f_contiguous:
         raise ValueError("out_states must be a Fortran-ordered (G, C) int32 or uint8 array")
@@ -221,16 +239,29 @@ def smooth_hmm(X, chr_start, chr_len, ref_groups, Pi, delta, mean, sd, apply_log
 
 
 def smooth_i3_hmm(X, chr_start, chr_len, ref_groups, i3_p_val=0.05, t=1e-6, median_lists=None, median_window=7,
-                  apply_log=True, threshold=3.0, window_length=101, use_bounds=True):
+                  apply_log=True, threshold=3.0, window_length=101, use_bounds=True, groups=None):
     """Fused i3 pass (icnv_smooth_i3_hmm_u8_f64): smooth block, the i3 model of the reference cells' smoothed values,
     per-cell i3 HMM and, with `median_lists`, apply_median_filtering(window = median_window) over those index lists, in one
-    pass over the matrix.  Returns (Y, states uint8, F or None, {"mu", "sigma", "mean_delta"})."""
+    pass over the matrix.  Returns (Y, states uint8, F or None, {"mu", "sigma", "mean_delta"}).
+
+    groups: the HMM lists of analysis_mode "samples" / "subclusters" (icnv_smooth_i3_hmm_groups_u8_f64): the group i3 HMM,
+    255 for cells in no group.  It has no median filter (F is None): run median_filter on Y."""
     X = _f64(X)
     G, C = X.shape
     cs, cl = _i32(chr_start), _i32(chr_len)
     off, idx = groups_to_csr(ref_groups)
     Y = np.empty_like(X, order="F")
     S = np.empty((G, C), dtype=np.uint8, order="F")
+    if groups is not None:
+        if median_lists is not None:
+            raise ValueError("the group-mode i3 pass has no median filter: run median_filter on Y")
+        hoff, hidx = groups_to_csr(groups)
+        model = np.zeros(3, dtype=np.float64)
+        _lib.check(_lib.load().icnv_smooth_i3_hmm_groups_u8_f64(
+            _p(X), _p(Y), _p(S), G, C, _p(cs), _p(cl), len(cs), _p(off), _p(idx), len(ref_groups), int(bool(apply_log)),
+            float(threshold), int(window_length), int(bool(use_bounds)), _p(hoff), _p(hidx), len(groups), float(i3_p_val),
+            float(t), _p(model)))
+        return Y, S, None, {"mu": float(model[0]), "sigma": float(model[1]), "mean_delta": float(model[2])}
     lists = [] if median_lists is None else list(median_lists)
     moff, midx = groups_to_csr(lists)
     F = np.empty_like(X, order="F") if median_lists is not None else None

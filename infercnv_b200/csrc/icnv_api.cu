@@ -65,6 +65,9 @@ namespace icnv {
 // K12 in either layout (icnv_dist.cu)
 int knn_launch(const double *X, int64_t G, int64_t ldx, const int32_t *d_cells, int64_t n, int k, int32_t *idx, double *dist,
                int rows, void *stream, const char *who);
+// K1 over a list-ordered slab (icnv_smooth.cu)
+int slab_group_sums(const double *Y, int64_t G, int64_t ldy, const int32_t *d_chunks, int64_t n_chunks, const int32_t *d_segs,
+                    int64_t n_segs, double *partial, const double *acc_in, double *acc_out, double *means, void *stream);
 }  // namespace icnv
 
 namespace icnv {
@@ -137,43 +140,51 @@ public:
         for (auto &t : th_) t.join();
     }
     int size() const { return n_; }
-    // copies up to two (dst, src, bytes) jobs, cut into equal byte ranges over the threads; returns when both are done
-    void copy2(void *d0, const void *s0, size_t n0, void *d1, const void *s1, size_t n1) {
-        if (n0 + n1 == 0) return;
-        std::unique_lock<std::mutex> lk(mu_);
-        job_[0] = {static_cast<char *>(d0), static_cast<const char *>(s0), n0};
-        job_[1] = {static_cast<char *>(d1), static_cast<const char *>(s1), n1};
-        pending_ = n_;
-        ++gen_;
-        cv_.notify_all();
-        done_.wait(lk, [this] { return pending_ == 0; });
-    }
-
-private:
     struct Job {
         char *d;
         const char *s;
         size_t n;
     };
+    // copies the (dst, src, bytes) jobs, their bytes laid end to end and cut into equal ranges over the threads; returns
+    // when every job is done
+    void copyv(const std::vector<Job> &jobs) {
+        size_t total = 0;
+        for (const Job &j : jobs) total += j.n;
+        if (total == 0) return;
+        std::unique_lock<std::mutex> lk(mu_);
+        job_ = &jobs;
+        pending_ = n_;
+        ++gen_;
+        cv_.notify_all();
+        done_.wait(lk, [this] { return pending_ == 0; });
+    }
+    void copy2(void *d0, const void *s0, size_t n0, void *d1, const void *s1, size_t n1) {
+        copyv({{static_cast<char *>(d0), static_cast<const char *>(s0), n0},
+               {static_cast<char *>(d1), static_cast<const char *>(s1), n1}});
+    }
+
+private:
     void loop(int t) {
         unsigned long long seen = 0;
         for (;;) {
-            Job j[2];
+            const std::vector<Job> *jobs;
             {
                 std::unique_lock<std::mutex> lk(mu_);
                 cv_.wait(lk, [&] { return gen_ != seen; });
                 seen = gen_;
                 if (stop_) return;
-                j[0] = job_[0];
-                j[1] = job_[1];
+                jobs = job_;
             }
-            const size_t total = j[0].n + j[1].n;
+            size_t total = 0;
+            for (const Job &j : *jobs) total += j.n;
             const size_t per = ((total + (size_t)n_ - 1) / (size_t)n_ + 4095) & ~(size_t)4095;
-            size_t lo = per * (size_t)t, hi = std::min(total, lo + per);
-            for (int k = 0; k < 2 && lo < hi; ++k) {   // the byte range [lo, hi) of job 0 followed by job 1
-                const size_t base = k == 0 ? 0 : j[0].n;
-                const size_t a = std::max(lo, base), b = std::min(hi, base + j[k].n);
-                if (a < b) stream_copy(j[k].d + (a - base), j[k].s + (a - base), b - a);
+            const size_t lo = per * (size_t)t, hi = std::min(total, lo + per);
+            size_t base = 0;
+            for (const Job &j : *jobs) {   // the byte range [lo, hi) of the jobs laid end to end
+                if (base >= hi) break;
+                const size_t a = std::max(lo, base), b = std::min(hi, base + j.n);
+                if (a < b) stream_copy(j.d + (a - base), j.s + (a - base), b - a);
+                base += j.n;
             }
             std::lock_guard<std::mutex> lk(mu_);
             if (--pending_ == 0) done_.notify_all();
@@ -183,7 +194,7 @@ private:
     std::vector<std::thread> th_;
     std::mutex mu_;
     std::condition_variable cv_, done_;
-    Job job_[2] = {};
+    const std::vector<Job> *job_ = nullptr;
     int pending_ = 0;
     unsigned long long gen_ = 0;
     bool stop_ = false;
@@ -753,6 +764,41 @@ struct I3Fused {
     }
 };
 
+/* What the fused group-mode calls change in the slab pipeline.  The cells go through it in HMM-list order - every list
+ * entry, then the cells in no list in column order - so that a group's 32-entry chunks (dev_group_means' summation tree)
+ * lie in one slab each: pipeline position p is column order[p].  Slabs gather their columns from X and scatter Y back,
+ * each column written from the one position that owns it (its last listing; an unlisted cell's own position).  The group
+ * means build up slab by slab; after the last slab the group Viterbi runs on them and every owned column of `states`
+ * takes its group's trace (255: in no list).  A device's positions start and end at group boundaries. */
+struct GroupHmm {
+    const int32_t *off;              // hmm_off[n_hmm + 1]
+    int n_hmm;
+    int64_t n_listed;                // off[n_hmm]
+    std::vector<int32_t> order;      // position -> column
+    std::vector<int32_t> grp_at;     // position -> its group (the listed positions)
+    std::vector<char> owns;          // position -> whether it writes its column's Y and states
+    std::vector<double> sd_med;      // i6: per-group median sd (viterbi_impl's); empty: i3 (sigma for every group)
+    uint8_t *states;
+    // the column of position p
+    int64_t col(int64_t p) const { return order[(size_t)p]; }
+    // the smallest position >= x at which a slab may end: a group boundary, a chunk boundary inside a group, or any
+    // position among the unlisted cells
+    bool may_cut(int64_t x) const {
+        if (x >= n_listed) return true;
+        return (x - off[grp_at[(size_t)x]]) % 32 == 0;
+    }
+    // the position nearest x that is a group boundary (ties: the lower one) - where the devices' shares are cut
+    int64_t group_cut_near(int64_t x) const {
+        if (x >= n_listed) return x;
+        const int k = grp_at[(size_t)x];
+        return (x - off[k] <= off[k + 1] - x) ? off[k] : off[k + 1];
+    }
+    // the first group whose entries start at or after position x
+    int group_at_or_after(int64_t x) const {
+        return (int)(std::lower_bound(off, off + n_hmm + 1, (int32_t)std::min<int64_t>(x, n_listed)) - off);
+    }
+};
+
 // Several devices: every device's range allocates its buffers first and waits here for the others, so that a range whose
 // buffers do not fit stops every device before any of them has written output.
 struct StartGate {
@@ -783,16 +829,18 @@ struct StartGate {
 // groups index the whole matrix (every device reduces all reference cells itself, in list order).
 // i3 (with do_smooth, hmm == NULL): the per-cell HMM uses the i3 model of the block's reference cells, and F (optional)
 // is the median filter of Y; [c_lo, c_hi) must not cut a list's span.
+// grp (with do_smooth, states == states8 == NULL, no F): the group-mode HMM of GroupHmm; [c_lo, c_hi) are pipeline positions
+// and start and end at group boundaries.
 static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *states, uint8_t *states8, int64_t G, int64_t c_lo,
                                int64_t c_hi, const int32_t *chr_start, const int32_t *chr_len, int K, int do_smooth,
                                const int32_t *grp_off, const int32_t *grp_idx, int n_grp, int apply_log, double threshold,
                                int window, int use_bounds, const HmmModel *hmm, CopyPool *pool, const I3Fused *i3 = nullptr,
-                               StartGate *gate = nullptr) {
+                               StartGate *gate = nullptr, const GroupHmm *grp = nullptr) {
     cudaStream_t sc = c.stream, sh = c.s_h2d, sd = c.s_d2h;
     int rc;
     const int64_t C = c_hi - c_lo;
     const bool mf = i3 && i3->F;
-    const bool has_hmm = hmm || i3;
+    const bool has_hmm = (hmm || i3) && !grp;   // the per-cell HMM, slab by slab
     int *d_flag = (int *)scratch(SLOT_MISC, 64);
     if (!d_flag) return ICNV_E_NOMEM;
     if (mf) d_flag += 4;   // icnv_dev_median_filter_f64 clears and sets the slot's first word for itself
@@ -818,13 +866,22 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     }
     if (c.opt_slab_cells) slab_cells = c.opt_slab_cells;
     const int64_t slab = std::max<int64_t>(1, std::min<int64_t>(slab_cells, C));
-    const size_t slab_elems = (size_t)G * (size_t)slab;
     // slab i is the cells [c_lo + s_at[i], c_lo + s_at[i + 1]).  With the median filter the slabs are cut inside units (see
     // I3Fused); unit_lo[i] is the first cell of slab i's unit, unit_end[i] marks its last slab.
     std::vector<int64_t> s_at{0}, unit_lo;
     std::vector<char> unit_end;
     int64_t max_unit = 0;
-    for (int64_t u0 = 0; u0 < C;) {
+    for (int64_t u0 = 0; grp && u0 < C;) {   // group mode: a slab ends where no 32-entry chunk is cut
+        int64_t q = std::min(C, u0 + slab);
+        while (!grp->may_cut(c_lo + q)) --q;
+        if (q == u0) {   // a slab shorter than a chunk: round up instead
+            q = u0 + 1;
+            while (!grp->may_cut(c_lo + q)) ++q;
+        }
+        s_at.push_back(q);
+        u0 = q;
+    }
+    for (int64_t u0 = 0; !grp && u0 < C;) {
         const int64_t u1 = mf ? std::min(C, i3->cut_at_or_after(c_lo + u0 + slab) - c_lo) : C;
         for (int64_t s = u0; s < u1; s += slab) {
             s_at.push_back(std::min(u1, s + slab));
@@ -834,6 +891,9 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         max_unit = std::max(max_unit, u1 - u0);
         u0 = u1;
     }
+    int64_t slab_cap = slab;
+    for (size_t i = 0; i + 1 < s_at.size(); ++i) slab_cap = std::max(slab_cap, s_at[i + 1] - s_at[i]);
+    const size_t slab_elems = (size_t)G * (size_t)slab_cap;
     double *dIn[2], *dOut[2] = {nullptr, nullptr};
     uint8_t *dSt[2] = {nullptr, nullptr};
     int32_t *dW[2] = {nullptr, nullptr};
@@ -872,9 +932,87 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     }
     const int64_t n_slabs = (int64_t)s_at.size() - 1;
     auto slab_cells_of = [&](int64_t i) { return s_at[(size_t)i + 1] - s_at[(size_t)i]; };
+    // group mode: runs of consecutive columns among slab i's positions, f(first slab column, first matrix column, length);
+    // owners_only: the positions that write their column
+    auto col_runs = [&](int64_t i, bool owners_only, const std::function<int(int64_t, int64_t, int64_t)> &f) -> int {
+        const int64_t p0 = c_lo + s_at[(size_t)i], p1 = c_lo + s_at[(size_t)i + 1];
+        for (int64_t p = p0; p < p1;) {
+            if (owners_only && !grp->owns[(size_t)p]) {
+                ++p;
+                continue;
+            }
+            int64_t q = p + 1;
+            while (q < p1 && (!owners_only || grp->owns[(size_t)q]) && grp->col(q) == grp->col(q - 1) + 1) ++q;
+            if (int rc2 = f(p - p0, grp->col(p), q - p)) return rc2;
+            p = q;
+        }
+        return ICNV_OK;
+    };
+    // group mode: this range's groups [k_lo, k_hi); per slab i its chunks [ch_at[i], ch_at[i + 1]) (pairs: first slab
+    // column, entries) and group segments [sg_at[i], sg_at[i + 1]) (see slab_combine_kernel), uploaded once
+    const int k_lo = grp ? grp->group_at_or_after(c_lo) : 0, k_hi = grp ? grp->group_at_or_after(c_hi) : 0;
+    const int64_t n_loc = k_hi - k_lo;
+    std::vector<int64_t> ch_at{0}, sg_at{0};
+    double *d_gm = nullptr, *d_gsd = nullptr, *d_part = nullptr;
+    int32_t *d_chunks = nullptr, *d_segs = nullptr;
+    uint8_t *d_gst = nullptr;
+    if (grp) {
+        std::vector<int32_t> chunks, segs;
+        int64_t max_ch = 1;
+        for (int64_t i = 0; i < n_slabs; ++i) {
+            const int64_t p0 = c_lo + s_at[(size_t)i], p1 = c_lo + s_at[(size_t)i + 1];
+            const int64_t first = (int64_t)chunks.size() / 2;
+            for (int k = p0 < grp->n_listed ? grp->grp_at[(size_t)p0] : grp->n_hmm; k < grp->n_hmm && grp->off[k] < p1; ++k) {
+                const int64_t a = grp->off[k], e = grp->off[k + 1];
+                const int64_t ch0 = (int64_t)chunks.size() / 2 - first;
+                for (int64_t q = std::max(a, p0); q < std::min(e, p1); q += 32) {   // max(a, p0) starts a chunk
+                    chunks.push_back((int32_t)(q - p0));
+                    chunks.push_back((int32_t)std::min<int64_t>(32, e - q));
+                }
+                segs.insert(segs.end(), {(int32_t)ch0, (int32_t)((int64_t)chunks.size() / 2 - first - ch0), a >= p0, e <= p1,
+                                         (int32_t)(e - a), (int32_t)(k - k_lo)});
+            }
+            ch_at.push_back((int64_t)chunks.size() / 2);
+            sg_at.push_back((int64_t)segs.size() / 6);
+            max_ch = std::max(max_ch, ch_at.back() - ch_at[ch_at.size() - 2]);
+        }
+        d_gm = (double *)scratch(SLOT_GRP_MEANS, sizeof(double) * ((size_t)G + 1) * (size_t)n_loc);
+        d_part = (double *)scratch(SLOT_GRP_PART, sizeof(double) * (size_t)G * (size_t)(max_ch + 2));
+        d_chunks = (int32_t *)scratch(SLOT_GRP_TAB, sizeof(int32_t) * (chunks.size() + segs.size()));
+        d_gst = (uint8_t *)scratch(SLOT_GRP_ST, (size_t)G * (size_t)n_loc);
+        if (!d_gm || !d_part || !d_chunks || !d_gst)
+            return set_error(ICNV_E_NOMEM, "group-mode HMM: the means, traces and slab tables of %lld groups do not fit on device "
+                             "%d: %s", (long long)n_loc, c.device, icnv_last_error());
+        d_gsd = d_gm + (size_t)G * (size_t)n_loc;
+        d_segs = d_chunks + chunks.size();
+        ICNV_CUDA(cudaMemcpyAsync(d_chunks, chunks.data(), sizeof(int32_t) * chunks.size(), cudaMemcpyHostToDevice, sc));
+        ICNV_CUDA(cudaMemcpyAsync(d_segs, segs.data(), sizeof(int32_t) * segs.size(), cudaMemcpyHostToDevice, sc));
+        ICNV_CUDA(cudaStreamSynchronize(sc));   // the tables are pageable host vectors
+    }
     // results of slab j leave the pinned ring for the caller's buffers (after its D2H has completed); together with the
     // input of slab `in` entering the ring when in >= 0 - one hand-over to the copy threads for both directions
     auto host_copies = [&](int64_t in, int64_t out) -> int {
+        if (grp) {   // the slab's columns gathered into the ring; Y scattered from it to the columns its positions own
+            std::vector<CopyPool::Job> jobs;
+            if (in >= 0 && in < n_slabs && stage_in) {
+                const int b = (int)(in & 1);
+                if (in >= 2) ICNV_CUDA(cudaEventSynchronize(c.ev_h2d[b]));
+                col_runs(in, false, [&](int64_t r, int64_t col, int64_t n) {
+                    jobs.push_back({(char *)(pIn[b] + G * r), (const char *)(X + G * col), sizeof(double) * (size_t)(G * n)});
+                    return ICNV_OK;
+                });
+            }
+            if (out >= 0 && out < n_slabs && stage_out) {
+                const int b = (int)(out & 1);
+                ICNV_CUDA(cudaEventSynchronize(c.ev_d2h[b]));
+                col_runs(out, true, [&](int64_t r, int64_t col, int64_t n) {
+                    jobs.push_back({(char *)(Y + G * col), (const char *)(pOut[b] + G * r), sizeof(double) * (size_t)(G * n)});
+                    return ICNV_OK;
+                });
+            }
+            pool->copyv(jobs);
+            return ICNV_OK;
+        }
         void *d0 = nullptr, *d1 = nullptr;
         const void *s0 = nullptr, *s1 = nullptr;
         size_t n0 = 0, n1 = 0;
@@ -918,8 +1056,16 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         const int b = (int)(i & 1);
         const int64_t c0 = c_lo + s_at[(size_t)i], nc = slab_cells_of(i);
         if (i >= 2) ICNV_CUDA(cudaStreamWaitEvent(sh, c.ev_comp[b], 0));
-        ICNV_CUDA(cudaMemcpyAsync(dIn[b], stage_in ? pIn[b] : X + G * c0, sizeof(double) * (size_t)G * (size_t)nc,
-                                  cudaMemcpyHostToDevice, sh));
+        if (grp && !stage_in) {   // page-locked X: one copy per run of consecutive columns
+            int rc2 = col_runs(i, false, [&](int64_t r, int64_t col, int64_t n) -> int {
+                ICNV_CUDA(cudaMemcpyAsync(dIn[b] + G * r, X + G * col, sizeof(double) * (size_t)(G * n), cudaMemcpyHostToDevice, sh));
+                return ICNV_OK;
+            });
+            if (rc2) return rc2;
+        } else {
+            ICNV_CUDA(cudaMemcpyAsync(dIn[b], stage_in ? pIn[b] : X + G * c0, sizeof(double) * (size_t)G * (size_t)nc,
+                                      cudaMemcpyHostToDevice, sh));
+        }
         ICNV_CUDA(cudaEventRecord(c.ev_h2d[b], sh));
         return ICNV_OK;
     };
@@ -1088,7 +1234,13 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
             if (rc) return rc;
             hmm_in = d_out;
         }
-        if (hmm) {
+        if (grp) {
+            rc = slab_group_sums(d_out, G, G, d_chunks + 2 * ch_at[(size_t)i], ch_at[(size_t)i + 1] - ch_at[(size_t)i],
+                                 d_segs + 6 * sg_at[(size_t)i], sg_at[(size_t)i + 1] - sg_at[(size_t)i], d_part + 2 * G,
+                                 d_part + G * (i & 1), d_part + G * ((i + 1) & 1), d_gm, sc);
+            if (rc) return rc;
+        }
+        if (has_hmm) {
             rc = icnv_dev_viterbi_f64(hmm_in, G, nc, chr_start, chr_len, K, hmm->m, hmm->Pi, hmm->delta, hmm->mean, hmm->sd,
                                       0, dSt[b], nullptr, d_flag, sc);
             if (rc) return rc;
@@ -1097,7 +1249,15 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
         ICNV_CUDA(cudaEventRecord(c.ev_comp[b], sc));
         // D2H (staged: the ring slot of slab i-2 was emptied by host_copies(.., i-2) below, two iterations ago)
         ICNV_CUDA(cudaStreamWaitEvent(sd, c.ev_comp[b], 0));
-        if (do_smooth && Y) ICNV_CUDA(cudaMemcpyAsync(stage_out ? pOut[b] : Y + G * c0, d_out, bytes, cudaMemcpyDeviceToHost, sd));
+        if (do_smooth && Y && grp && !stage_out) {   // page-locked Y: one copy per run of owned consecutive columns
+            rc = col_runs(i, true, [&](int64_t r, int64_t col, int64_t n) -> int {
+                ICNV_CUDA(cudaMemcpyAsync(Y + G * col, d_out + G * r, sizeof(double) * (size_t)(G * n), cudaMemcpyDeviceToHost, sd));
+                return ICNV_OK;
+            });
+            if (rc) return rc;
+        } else if (do_smooth && Y) {
+            ICNV_CUDA(cudaMemcpyAsync(stage_out ? pOut[b] : Y + G * c0, d_out, bytes, cudaMemcpyDeviceToHost, sd));
+        }
         if (hmm && states)
             ICNV_CUDA(cudaMemcpyAsync(stage_out ? (int32_t *)pSt[b] : states + G * c0, dW[b],
                                       sizeof(int32_t) * (size_t)G * (size_t)nc, cudaMemcpyDeviceToHost, sd));
@@ -1113,7 +1273,30 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
     if (stage_out && (rc = host_copies(-1, n_slabs - 1))) return rc;
     ICNV_CUDA(cudaStreamSynchronize(sh));
     ICNV_CUDA(cudaStreamSynchronize(sd));
-    return check_flag(d_flag, sc);
+    if (!grp) return check_flag(d_flag, sc);
+
+    // group mode: the Viterbi of this range's groups (viterbi_impl's per-group median sd; i3: sigma), then every column its
+    // positions own takes its group's trace, 255 for the cells in no list
+    std::vector<uint8_t> h_st((size_t)G * (size_t)n_loc);
+    std::vector<double> sdl((size_t)n_loc);
+    if (n_loc > 0) {
+        for (int64_t j = 0; j < n_loc; ++j) sdl[(size_t)j] = grp->sd_med.empty() ? hmm->sd[0] : grp->sd_med[(size_t)(k_lo + j)];
+        ICNV_CUDA(cudaMemcpyAsync(d_gsd, sdl.data(), sizeof(double) * (size_t)n_loc, cudaMemcpyHostToDevice, sc));
+        rc = icnv_dev_viterbi_f64(d_gm, G, n_loc, chr_start, chr_len, K, hmm->m, hmm->Pi, hmm->delta, hmm->mean, d_gsd, 1, d_gst,
+                                  nullptr, d_flag, sc);
+        if (rc) return rc;
+        ICNV_CUDA(cudaMemcpyAsync(h_st.data(), d_gst, h_st.size(), cudaMemcpyDeviceToHost, sc));
+    }
+    if ((rc = check_flag(d_flag, sc))) return rc;
+    const std::vector<uint8_t> none((size_t)G, 255);
+    std::vector<CopyPool::Job> jobs;
+    for (int64_t p = c_lo; p < c_hi; ++p) {
+        if (!grp->owns[(size_t)p]) continue;
+        const uint8_t *src = p < grp->n_listed ? h_st.data() + (size_t)G * (size_t)(grp->grp_at[(size_t)p] - k_lo) : none.data();
+        jobs.push_back({(char *)(grp->states + G * grp->col(p)), (const char *)src, (size_t)G});
+    }
+    pool->copyv(jobs);
+    return ICNV_OK;
 }
 
 // The cells are cut into one contiguous range per device context; each range is driven by its own host thread (a CUDA
@@ -1121,21 +1304,24 @@ static int host_pipeline_range(Ctx &c, const double *X, double *Y, int32_t *stat
 static int host_pipeline(Ctx &c0, const double *X, double *Y, int32_t *states, uint8_t *states8, int64_t G, int64_t C,
                          const int32_t *chr_start, const int32_t *chr_len, int K, int do_smooth, const int32_t *grp_off,
                          const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window, int use_bounds,
-                         const HmmModel *hmm, const I3Fused *i3 = nullptr) {
+                         const HmmModel *hmm, const I3Fused *i3 = nullptr, const GroupHmm *grp = nullptr) {
+    // (group mode: C counts pipeline positions, see GroupHmm)
     const int n_dev = (int)std::min<int64_t>(std::max(1, device_slots()), std::max<int64_t>(1, C / 64));
     const bool pageable = !is_pinned(X) || (Y && !is_pinned(Y)) || (states && !is_pinned(states)) || (states8 && !is_pinned(states8)) ||
                           (i3 && i3->F && !is_pinned(i3->F));
     const int nt = pool_threads_per_device();
-    if (n_dev <= 1) {
-        std::unique_ptr<CopyPool> pool(pageable ? new CopyPool(nt) : nullptr);
+    if (n_dev <= 1) {   // (group mode: the copy threads also place the traces)
+        std::unique_ptr<CopyPool> pool(pageable || grp ? new CopyPool(nt) : nullptr);
         return host_pipeline_range(c0, X, Y, states, states8, G, 0, C, chr_start, chr_len, K, do_smooth, grp_off, grp_idx, n_grp,
-                                   apply_log, threshold, window, use_bounds, hmm, pool.get(), i3);
+                                   apply_log, threshold, window, use_bounds, hmm, pool.get(), i3, nullptr, grp);
     }
-    // even shares; with the median filter each cut moves to the nearest column no list's span crosses
+    // even shares; with the median filter each cut moves to the nearest column no list's span crosses, in group mode to the
+    // nearest group boundary (each group's means and trace come from one device)
     std::vector<int64_t> cut((size_t)n_dev + 1);
     for (int d = 0; d <= n_dev; ++d) {
         cut[(size_t)d] = C * d / n_dev;
         if (i3 && i3->F) cut[(size_t)d] = std::max(d ? cut[(size_t)d - 1] : 0, i3->cut_near(cut[(size_t)d]));
+        if (grp) cut[(size_t)d] = std::max(d ? cut[(size_t)d - 1] : 0, grp->group_cut_near(cut[(size_t)d]));
     }
     int reporter = 0;   // the first device with cells reports the i3 model (every device computes the same bits)
     while (reporter < n_dev - 1 && cut[(size_t)reporter] == cut[(size_t)reporter + 1]) ++reporter;
@@ -1152,7 +1338,7 @@ static int host_pipeline(Ctx &c0, const double *X, double *Y, int32_t *states, u
     int n_busy = 0;
     for (int d = 0; d < n_dev; ++d) n_busy += cut[(size_t)d] < cut[(size_t)d + 1];
     // the fused i3 call promises that a unit that does not fit is refused before any output is written
-    std::unique_ptr<StartGate> gate(i3 && i3->F ? new StartGate(n_dev, n_busy) : nullptr);
+    std::unique_ptr<StartGate> gate((i3 && i3->F) || grp ? new StartGate(n_dev, n_busy) : nullptr);
     for (int d = 0; d < n_dev; ++d) {
         const int64_t lo = cut[(size_t)d], hi = cut[(size_t)d + 1];
         if (lo == hi) continue;
@@ -1164,10 +1350,10 @@ static int host_pipeline(Ctx &c0, const double *X, double *Y, int32_t *states, u
             int rc = ICNV_OK;
             if (cudaSetDevice(c.device) != cudaSuccess) rc = set_error(ICNV_E_CUDA, "cudaSetDevice(%d) failed", c.device);
             if (!rc) {
-                std::unique_ptr<CopyPool> pool(pageable ? new CopyPool(nt) : nullptr);
+                std::unique_ptr<CopyPool> pool(pageable || grp ? new CopyPool(nt) : nullptr);
                 rc = host_pipeline_range(c, X, Y, states, states8, G, lo, hi, chr_start, chr_len, K, do_smooth, grp_off, grp_idx,
                                          n_grp, apply_log, threshold, window, use_bounds, hmm, pool.get(),
-                                         i3 ? &i3d[(size_t)d] : nullptr, gate.get());
+                                         i3 ? &i3d[(size_t)d] : nullptr, gate.get(), grp);
             }
             if (gate) gate->arrive(d, rc == ICNV_OK);   // a range that failed before the gate still has to open it
             rcs[(size_t)d] = rc;
@@ -1268,6 +1454,84 @@ int icnv_smooth_i3_hmm_u8_f64(const double *X, double *Y, uint8_t *states, doubl
     }
     return host_pipeline(c, X, Y, nullptr, states, G, C, chr_start, chr_len, K, 1, grp_off, grp_idx, n_grp, apply_log, threshold,
                          window, use_bounds, nullptr, &i3);
+}
+
+// The pipeline order of the group-mode calls (see GroupHmm) from the HMM lists; BAD_ARG for n_hmm == 0 or a bad list.
+static int group_hmm_order(GroupHmm &gh, int64_t C, const int32_t *hmm_off, const int32_t *hmm_idx, int n_hmm, uint8_t *states) {
+    if (n_hmm == 0) return set_error(ICNV_E_BAD_ARG, "n_hmm == 0: the per-cell calls run the HMM without groups");
+    int rc = validate_groups(C, hmm_off, hmm_idx, n_hmm, false);
+    if (rc) return rc;
+    gh.off = hmm_off;
+    gh.n_hmm = n_hmm;
+    gh.n_listed = hmm_off[n_hmm];
+    gh.states = states;
+    std::vector<int32_t> last((size_t)C, -1);   // a cell's last listing writes it, as viterbi_impl's grp_of
+    for (int32_t p = 0; p < hmm_off[n_hmm]; ++p) last[(size_t)hmm_idx[p]] = p;
+    gh.order.assign(hmm_idx, hmm_idx + gh.n_listed);
+    gh.grp_at.resize((size_t)gh.n_listed);
+    gh.owns.resize((size_t)gh.n_listed);
+    for (int k = 0; k < n_hmm; ++k)
+        for (int32_t p = hmm_off[k]; p < hmm_off[k + 1]; ++p) {
+            gh.grp_at[(size_t)p] = k;
+            gh.owns[(size_t)p] = last[(size_t)hmm_idx[p]] == p;
+        }
+    for (int64_t c = 0; c < C; ++c)
+        if (last[(size_t)c] < 0) {
+            gh.order.push_back((int32_t)c);
+            gh.owns.push_back(1);
+        }
+    return ICNV_OK;
+}
+
+/* Fused smooth block + group-mode HMM (see the header): run() steps 4..14 and 17 for analysis_mode "samples" and
+ * "subclusters" (random_trees), one read of X and one write of Y and states. */
+int icnv_smooth_hmm_groups_u8_f64(const double *X, double *Y, uint8_t *states, int64_t G, int64_t C, const int32_t *chr_start,
+                                  const int32_t *chr_len, int K, const int32_t *grp_off, const int32_t *grp_idx, int n_grp,
+                                  int apply_log, double threshold, int window, int use_bounds, const int32_t *hmm_off,
+                                  const int32_t *hmm_idx, int n_hmm, int m, const double *Pi, const double *delta,
+                                  const double *mean, const double *sd) {
+    ICNV_HOST_PROLOGUE();
+    if (!X || !Y || !states || G <= 0 || C <= 0 || !Pi || !delta || !mean || !sd)
+        return set_error(ICNV_E_BAD_ARG, "icnv_smooth_hmm_groups_u8_f64: bad argument");
+    if (m != 6 && m != 3) return set_error(ICNV_E_BAD_ARG, "m must be 6 or 3");
+    int rc = validate_chr(G, chr_start, chr_len, K);
+    if (rc) return rc;
+    if ((rc = validate_groups(C, grp_off, grp_idx, n_grp, false))) return rc;
+    GroupHmm gh;
+    if ((rc = group_hmm_order(gh, C, hmm_off, hmm_idx, n_hmm, states))) return rc;
+    gh.sd_med.resize((size_t)n_hmm);
+    for (int b = 0; b < n_hmm; ++b) {   // viterbi_impl's per-group median sd
+        std::vector<double> v(sd + (size_t)m * b, sd + (size_t)m * (b + 1));
+        std::sort(v.begin(), v.end());
+        gh.sd_med[(size_t)b] = (m & 1) ? v[m / 2] : 0.5 * (v[m / 2 - 1] + v[m / 2]);
+        if (!(gh.sd_med[(size_t)b] > 0.0)) return set_error(ICNV_E_BAD_ARG, "state sd must be positive (group %d)", b);
+    }
+    HmmModel hm{m, Pi, delta, mean, sd};
+    return host_pipeline(c, X, Y, nullptr, nullptr, G, (int64_t)gh.order.size(), chr_start, chr_len, K, 1, grp_off, grp_idx,
+                         n_grp, apply_log, threshold, window, use_bounds, &hm, nullptr, &gh);
+}
+
+/* The i3 twin: the i3 model fixed from the block's reference cells as in icnv_smooth_i3_hmm_u8_f64, then the group-mode
+ * i3 HMM (sigma for every group).  No median filter. */
+int icnv_smooth_i3_hmm_groups_u8_f64(const double *X, double *Y, uint8_t *states, int64_t G, int64_t C,
+                                     const int32_t *chr_start, const int32_t *chr_len, int K, const int32_t *grp_off,
+                                     const int32_t *grp_idx, int n_grp, int apply_log, double threshold, int window,
+                                     int use_bounds, const int32_t *hmm_off, const int32_t *hmm_idx, int n_hmm,
+                                     double i3_p_val, double t, double *model) {
+    ICNV_HOST_PROLOGUE();
+    if (!X || !Y || !states || !model || G <= 1 || C <= 0)
+        return set_error(ICNV_E_BAD_ARG, "icnv_smooth_i3_hmm_groups_u8_f64: bad argument");
+    if (!(i3_p_val > 0.0 && i3_p_val < 1.0)) return set_error(ICNV_E_BAD_ARG, "i3_p_val must lie in (0, 1)");
+    if (window >= 2 && (window & 1) == 0)
+        return set_error(ICNV_E_BAD_ARG, "window_length %d is even: the reference's behaviour is accidental there", window);
+    int rc = validate_chr(G, chr_start, chr_len, K);
+    if (rc) return rc;
+    if ((rc = validate_groups(C, grp_off, grp_idx, n_grp, false))) return rc;
+    GroupHmm gh;
+    if ((rc = group_hmm_order(gh, C, hmm_off, hmm_idx, n_hmm, states))) return rc;
+    I3Fused i3{i3_p_val, t, model, nullptr, nullptr, nullptr, 0, 0, {}};
+    return host_pipeline(c, X, Y, nullptr, nullptr, G, (int64_t)gh.order.size(), chr_start, chr_len, K, 1, grp_off, grp_idx,
+                         n_grp, apply_log, threshold, window, use_bounds, nullptr, &i3, &gh);
 }
 
 static int viterbi_impl(const double *X, int64_t G, int64_t C, const int32_t *chr_start, const int32_t *chr_len, int K,

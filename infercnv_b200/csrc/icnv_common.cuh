@@ -51,6 +51,10 @@ enum ScratchSlot {
     SLOT_VIT_ITEMS,                   // chromosome work items of the Viterbi launch (cached: Ctx::up_items)
     SLOT_MF_PRE,                      // median filter: range of the matrix and the value sample of its pre-pass
     SLOT_KNN,                         // k nearest neighbours: per-split partial lists and the non-finite flag
+    SLOT_GRP_MEANS,                   // fused group-mode HMM: G x n_hmm group means, then the per-group sds
+    SLOT_GRP_PART,                    // ... chunk sums of one slab and the two sums of a group left open between slabs
+    SLOT_GRP_TAB,                     // ... chunk and segment tables of every slab
+    SLOT_GRP_ST,                      // ... uint8 G x n_hmm traces
     SLOT_COUNT
 };
 

@@ -76,6 +76,50 @@ __global__ void __launch_bounds__(256) combine_partials_kernel(const double *__r
     means[g] = s / inv_count_num;  // a true division by the count, as mean() does
 }
 
+// The two kernels above for a slab of columns in list order (the fused group-mode HMM): one launch per slab over every
+// 32-entry chunk in it, whatever group it belongs to.  chunks[2q] is the chunk's first slab column, chunks[2q + 1] its
+// entry count; the sum runs add for add as group_partial_sums_kernel's with apply_log = 0.
+__global__ void __launch_bounds__(256) slab_chunk_sums_kernel(const double *__restrict__ X, int64_t G, int64_t ldx,
+                                                              const int32_t *__restrict__ chunks, int64_t n_chunks,
+                                                              double *__restrict__ partial) {
+    int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    for (int64_t q = blockIdx.y; q < n_chunks; q += gridDim.y) {
+        const double *x = X + g + ldx * (int64_t)chunks[2 * q];
+        const int n = chunks[2 * q + 1];
+        double s = 0.0;
+        int i = 0;
+        for (; i + 4 <= n; i += 4) {
+            double v0 = x[ldx * i], v1 = x[ldx * (i + 1)], v2 = x[ldx * (i + 2)], v3 = x[ldx * (i + 3)];
+            s += v0;
+            s += v1;
+            s += v2;
+            s += v3;
+        }
+        for (; i < n; ++i) s += x[ldx * i];
+        partial[g + G * q] = s;
+    }
+}
+
+// combine_partials_kernel for every group segment of a slab.  segs[6 k ..] = first chunk, chunk count, opens, closes, group
+// size, means column.  A segment that does not open continues the sum of the group left open by the previous slab (acc_in);
+// one that does not close leaves its sum for the next slab (acc_out).  Only the last group of a slab can stay open, and
+// acc_in != acc_out, so no two segments of a launch touch the same word.
+__global__ void __launch_bounds__(256) slab_combine_kernel(const double *__restrict__ partial, int64_t G,
+                                                           const int32_t *__restrict__ segs, int64_t n_segs,
+                                                           const double *__restrict__ acc_in, double *__restrict__ acc_out,
+                                                           double *__restrict__ means) {
+    int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    for (int64_t k = blockIdx.y; k < n_segs; k += gridDim.y) {
+        const int32_t *sg = segs + 6 * k;
+        double s = sg[2] ? 0.0 : acc_in[g];
+        for (int q = 0; q < sg[1]; ++q) s += partial[g + G * (int64_t)(sg[0] + q)];
+        if (sg[3]) means[g + G * (int64_t)sg[5]] = s / (double)sg[4];
+        else acc_out[g] = s;
+    }
+}
+
 __global__ void __launch_bounds__(256) bounds_from_means_kernel(const double *__restrict__ means, int64_t G, int n_grp,
                                                                 double *__restrict__ lo, double *__restrict__ hi,
                                                                 double *__restrict__ mid) {
@@ -1694,6 +1738,20 @@ static int build_segments(int64_t G, const int32_t *chr_start, const int32_t *ch
         }
     }
     return 0;  // does not fit
+}
+
+// Group means of one list-ordered slab: the chunk sums, then every group segment of the slab (see the kernels).
+int slab_group_sums(const double *Y, int64_t G, int64_t ldy, const int32_t *d_chunks, int64_t n_chunks, const int32_t *d_segs,
+                    int64_t n_segs, double *partial, const double *acc_in, double *acc_out, double *means, void *stream) {
+    if (n_chunks == 0) return ICNV_OK;
+    const unsigned gx = (unsigned)((G + 255) / 256);
+    slab_chunk_sums_kernel<<<dim3(gx, (unsigned)std::min<int64_t>(n_chunks, 65535)), 256, 0, pick_stream(stream)>>>(
+        Y, G, ldy, d_chunks, n_chunks, partial);
+    ICNV_CHECK_LAUNCH("slab_chunk_sums_kernel");
+    slab_combine_kernel<<<dim3(gx, (unsigned)std::min<int64_t>(n_segs, 65535)), 256, 0, pick_stream(stream)>>>(
+        partial, G, d_segs, n_segs, acc_in, acc_out, means);
+    ICNV_CHECK_LAUNCH("slab_combine_kernel");
+    return ICNV_OK;
 }
 
 }  // namespace icnv

@@ -413,9 +413,16 @@ b200_get_predicted_CNV_regions <- function(infercnv_obj, by=c("consensus", "subc
 ## Returns list(infercnv_obj = <after step 14>, hmm_obj = <states object or NULL>), on the i3 path also median_obj (the
 ## median-filtered object or NULL) and sd_trend (.i3HMM_get_sd_trend_by_num_cells_fit's list); NULL when the input is outside
 ## the GPU path's envelope (the caller then runs the R steps).
+## analysis_mode = "samples" or "subclusters" (cluster_by_groups and tumor_subcluster_partition_method as in run()) runs
+## step 17 in group mode instead: i6 when i3_p_val is NULL (HMM_info is not read: the model and every group's sds come from
+## the smoothed hspike, as predict_CNV_via_HMM_on_whole_tumor_samples / _on_tumor_subclusters build them), i3 otherwise.
+## "subclusters" needs the random_trees partition, which run() makes at step 7, before the block; without subclusters on the
+## object the groups are the whole samples, as in R.  Leiden and the other partitions are made from the block's output: NULL.
+## The group-mode call has no median filter (median_obj is NULL; run b200_apply_median_filtering on infercnv_obj).
 infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_centered_threshold=3, use_bounds=TRUE,
                                           apply_log=TRUE, HMM_info=NULL, i3_p_val=NULL, t=1e-6, use_KS=FALSE,
-                                          median_filter_window=NULL) {
+                                          median_filter_window=NULL, analysis_mode="cells", cluster_by_groups=TRUE,
+                                          tumor_subcluster_partition_method="random_trees") {
     m <- infercnv_obj@expr.data
     codes <- .icnv_chr_codes(infercnv_obj)
     i3 <- is.null(HMM_info) && !is.null(i3_p_val)
@@ -427,6 +434,12 @@ infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_c
                                      if (i3) paste0(" + i3 model + per-cell HMM", if (is.null(median_filter_window)) "" else " + median filter")
                                      else if (is.null(HMM_info)) "" else " + per-cell HMM"))
     refs <- .icnv_ref_groups(infercnv_obj)
+    if (!identical(analysis_mode, "cells")) {
+        if (!(analysis_mode %in% c("samples", "subclusters")) || (!i3 && is.null(infercnv_obj@.hspike)) ||
+            (analysis_mode == "subclusters" && !identical(tumor_subcluster_partition_method, "random_trees"))) return(NULL)
+        return(.icnv_smooth_block_groups(infercnv_obj, m, codes, refs, window_length, max_centered_threshold, use_bounds,
+                                         apply_log, i3, i3_p_val, t, analysis_mode, cluster_by_groups))
+    }
     hmm_obj <- NULL
     median_obj <- NULL
     sd_trend <- NULL
@@ -478,6 +491,63 @@ infercnvb200_run_smooth_block <- function(infercnv_obj, window_length=101, max_c
         infercnv_obj@.hspike <- h$infercnv_obj
     }
     if (i3) return(list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj, median_obj = median_obj, sd_trend = sd_trend))
+    list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj)
+}
+
+## The HMM lists of predict_CNV_via_HMM_on_tumor_subclusters (unlist(tumor_subclusters$subclusters)) and
+## predict_CNV_via_HMM_on_whole_tumor_samples (observation groups - one cell each when cluster_by_groups is FALSE - then the
+## reference groups), R/inferCNV_HMM.R:345-567.
+.icnv_hmm_groups <- function(infercnv_obj, analysis_mode, cluster_by_groups) {
+    if (analysis_mode == "subclusters" && !is.null(infercnv_obj@tumor_subclusters))
+        return(lapply(unlist(infercnv_obj@tumor_subclusters[["subclusters"]], recursive=FALSE), as.integer))
+    if (analysis_mode == "subclusters") cluster_by_groups <- TRUE
+    obs <- if (isTRUE(cluster_by_groups)) infercnv_obj@observation_grouped_cell_indices
+           else as.list(unlist(infercnv_obj@observation_grouped_cell_indices))
+    lapply(c(obs, infercnv_obj@reference_grouped_cell_indices), as.integer)
+}
+
+## infercnvb200_run_smooth_block's group-mode path.  The hspike is smoothed first (its own small call), because the i6 sds
+## are fitted on the smoothed hspike: get_spike_dists, get_hspike_cnv_mean_sd_trend_by_num_cells_fit (which draws from R's
+## RNG), .get_HMM and .get_state_emission_params run here in the order the reference's drivers evaluate them at step 17 -
+## nothing between steps 14 and 17 draws in these modes - and the fused call follows.  The i3 path draws the KS delta as
+## the per-cell path does.
+.icnv_smooth_block_groups <- function(infercnv_obj, m, codes, refs, window_length, max_centered_threshold, use_bounds,
+                                      apply_log, i3, i3_p_val, t, analysis_mode, cluster_by_groups) {
+    futile.logger::flog.info(sprintf("::smooth block (steps 4, 8-12, 14) + %s HMM on %s in one pass (GPU)",
+                                     if (i3) "i3" else "i6", analysis_mode))
+    hmm_groups <- .icnv_hmm_groups(infercnv_obj, analysis_mode, cluster_by_groups)
+    if (!is.null(infercnv_obj@.hspike)) {
+        futile.logger::flog.info("-mirroring for hspike")
+        h <- infercnvb200_run_smooth_block(infercnv_obj@.hspike, window_length, max_centered_threshold, use_bounds, apply_log, NULL)
+        if (is.null(h)) return(NULL)
+        infercnv_obj@.hspike <- h$infercnv_obj
+    }
+    sd_trend <- NULL
+    if (i3) {
+        res <- .icnv_try(.Call("icnvR_smooth_i3_hmm_groups", m, codes, refs, isTRUE(apply_log), as.double(max_centered_threshold),
+                               as.integer(window_length), isTRUE(use_bounds), hmm_groups, as.double(i3_p_val), as.double(t)),
+                         "smooth_i3_hmm_groups")
+        if (is.null(res)) return(NULL)
+        mu <- res[[3]][1]; sigma <- res[[3]][2]; mean_delta <- res[[3]][3]
+        message("mean_delta: ", mean_delta, ", at sigma: ", sigma, ", and pval: ", i3_p_val)
+        KS_delta <- infercnv:::get_HoneyBADGER_setGexpDev(gexp.sd=sigma, alpha=i3_p_val, k_cells=length(unlist(refs)))
+        message("KS_delta: ", KS_delta, ", at sigma: ", sigma, ", and pval: ", i3_p_val)
+        sd_trend <- list(mu=mu, sigma=sigma, mean_delta=mean_delta, KS_delta=KS_delta)
+    } else {
+        cnv_mean_sd <- infercnv:::get_spike_dists(infercnv_obj@.hspike)
+        HMM_info <- infercnv:::.get_HMM(cnv_mean_sd, t)
+        fit <- infercnv:::get_hspike_cnv_mean_sd_trend_by_num_cells_fit(infercnv_obj@.hspike)
+        sds <- unlist(lapply(hmm_groups, function(g)
+            as.double(infercnv:::.get_state_emission_params(length(g), cnv_mean_sd, fit)$sd)))
+        res <- .icnv_try(.Call("icnvR_smooth_hmm_groups", m, codes, refs, isTRUE(apply_log), as.double(max_centered_threshold),
+                               as.integer(window_length), isTRUE(use_bounds), hmm_groups, HMM_info[["state_transitions"]],
+                               HMM_info[["delta"]], HMM_info[["state_emission_params"]]$mean, sds), "smooth_hmm_groups")
+        if (is.null(res)) return(NULL)
+    }
+    infercnv_obj@expr.data <- .icnv_keep_names(res[[1]], m)
+    hmm_obj <- infercnv_obj
+    hmm_obj@expr.data <- .icnv_keep_names(res[[2]], m)
+    if (i3) return(list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj, median_obj = NULL, sd_trend = sd_trend))
     list(infercnv_obj = infercnv_obj, hmm_obj = hmm_obj)
 }
 

@@ -193,6 +193,59 @@ SEXP icnvR_smooth_i3_hmm(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_
     return ans;
 }
 
+/* the group-mode twins (icnv_smooth_hmm_groups_u8_f64, icnv_smooth_i3_hmm_groups_u8_f64): run() steps 4, 8-12, 14 and
+ * step 17 for analysis_mode "samples" / "subclusters" on the HMM lists hmm_groups.  i6: Pi, delta, mean and sd (m entries
+ * per group); i3: i3_p_val and t.  Returns list(expr, states) (i6) or list(expr, states, c(mu, sigma, mean_delta)). */
+static SEXP smooth_hmm_groups(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_log, SEXP threshold, SEXP window_length,
+                              SEXP use_bounds, SEXP hmm_groups, int i3, SEXP Pi, SEXP delta, SEXP mean, SEXP sd, SEXP i3_p_val,
+                              SEXP t) {
+    SEXP dim = Rf_getAttrib(expr, R_DimSymbol);
+    int64_t G = INTEGER(dim)[0], C = INTEGER(dim)[1];
+    int32_t *cs = NULL, *cl = NULL, *off = NULL, *idx = NULL, *hoff = NULL, *hidx = NULL;
+    int K = chr_to_ranges(chr_codes, &cs, &cl);
+    int n_grp = list_to_csr(ref_groups, &off, &idx);
+    int n_hmm = list_to_csr(hmm_groups, &hoff, &hidx);
+    uint8_t *st = (uint8_t *)malloc((size_t)(G * C));
+    SEXP ans = PROTECT(Rf_allocVector(VECSXP, i3 ? 3 : 2));
+    SEXP y = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    SEXP states = PROTECT(Rf_allocMatrix(REALSXP, (int)G, (int)C));
+    SEXP model = PROTECT(Rf_allocVector(REALSXP, 3));
+    int rc;
+    if (K < 0 || n_grp < 0 || n_hmm < 0 || !st)
+        rc = ICNV_E_NOMEM;
+    else if (i3)
+        rc = icnv_smooth_i3_hmm_groups_u8_f64(REAL(expr), REAL(y), st, G, C, cs, cl, K, off, idx, n_grp, Rf_asLogical(apply_log),
+                                              Rf_asReal(threshold), Rf_asInteger(window_length), Rf_asLogical(use_bounds), hoff,
+                                              hidx, n_hmm, Rf_asReal(i3_p_val), Rf_asReal(t), REAL(model));
+    else
+        rc = icnv_smooth_hmm_groups_u8_f64(REAL(expr), REAL(y), st, G, C, cs, cl, K, off, idx, n_grp, Rf_asLogical(apply_log),
+                                           Rf_asReal(threshold), Rf_asInteger(window_length), Rf_asLogical(use_bounds), hoff, hidx,
+                                           n_hmm, Rf_length(delta), REAL(Pi), REAL(delta), REAL(mean), REAL(sd));
+    if (rc == 0) {
+        double *out = REAL(states);   /* the reference keeps states as doubles; -1 for cells in no group */
+        for (int64_t i = 0; i < G * C; ++i) out[i] = (st[i] == 255) ? -1.0 : (double)st[i];
+    }
+    SET_VECTOR_ELT(ans, 0, y);
+    SET_VECTOR_ELT(ans, 1, states);
+    if (i3) SET_VECTOR_ELT(ans, 2, model);
+    free(cs); free(cl); free(off); free(idx); free(hoff); free(hidx); free(st);
+    UNPROTECT(4);
+    fail_if(rc);
+    return ans;
+}
+
+SEXP icnvR_smooth_hmm_groups(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_log, SEXP threshold, SEXP window_length,
+                             SEXP use_bounds, SEXP hmm_groups, SEXP Pi, SEXP delta, SEXP mean, SEXP sd) {
+    return smooth_hmm_groups(expr, chr_codes, ref_groups, apply_log, threshold, window_length, use_bounds, hmm_groups, 0, Pi,
+                             delta, mean, sd, R_NilValue, R_NilValue);
+}
+
+SEXP icnvR_smooth_i3_hmm_groups(SEXP expr, SEXP chr_codes, SEXP ref_groups, SEXP apply_log, SEXP threshold,
+                                SEXP window_length, SEXP use_bounds, SEXP hmm_groups, SEXP i3_p_val, SEXP t) {
+    return smooth_hmm_groups(expr, chr_codes, ref_groups, apply_log, threshold, window_length, use_bounds, hmm_groups, 1,
+                             R_NilValue, R_NilValue, R_NilValue, R_NilValue, i3_p_val, t);
+}
+
 /* icnv_init_devices: single-process multi-GPU (infercnv::run() is one R process).  ids = NULL: every GPU present. */
 SEXP icnvR_init_devices(SEXP ids) {
     int rc = Rf_isNull(ids) ? icnv_init_devices(0, NULL) : icnv_init_devices(Rf_length(ids), INTEGER(ids));
@@ -794,6 +847,8 @@ static const R_CallMethodDef call_methods[] = {
     {"icnvR_clear_noise_threshold", (DL_FUNC)&icnvR_clear_noise_threshold, 4},
     {"icnvR_smooth_hmm", (DL_FUNC)&icnvR_smooth_hmm, 11},   {"icnvR_init_devices", (DL_FUNC)&icnvR_init_devices, 1},
     {"icnvR_smooth_i3_hmm", (DL_FUNC)&icnvR_smooth_i3_hmm, 11},
+    {"icnvR_smooth_hmm_groups", (DL_FUNC)&icnvR_smooth_hmm_groups, 12},
+    {"icnvR_smooth_i3_hmm_groups", (DL_FUNC)&icnvR_smooth_i3_hmm_groups, 10},
     {"icnvR_pairwise_dist", (DL_FUNC)&icnvR_pairwise_dist, 1}, {"icnvR_hclust", (DL_FUNC)&icnvR_hclust, 2},
     {"icnvR_knn", (DL_FUNC)&icnvR_knn, 2},
     {"icnvR_runmean", (DL_FUNC)&icnvR_runmean, 4},

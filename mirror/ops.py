@@ -225,14 +225,62 @@ def smooth_block(infercnv_obj: Infercnv, window_length: int = 101, max_centered_
     return obj
 
 
+def _hmm_groups(obj: Infercnv, analysis_mode: str, cluster_by_groups: bool) -> list:
+    """The HMM lists of the group-mode drivers: unlist(tumor_subclusters$subclusters) for "subclusters"
+    (predict_CNV_via_HMM_on_tumor_subclusters, HMM.R:345-408; without subclusters R falls back to whole samples with
+    cluster_by_groups = TRUE), else the observation groups - one-cell groups when cluster_by_groups is FALSE - then the
+    reference groups (..._on_whole_tumor_samples, HMM.R:509-567)."""
+    if analysis_mode not in ("samples", "subclusters"):
+        raise ValueError(f"analysis_mode {analysis_mode!r} has no HMM groups")
+    if analysis_mode == "subclusters":
+        if obj.tumor_subclusters is not None:
+            return [np.asarray(idx) for sub in obj.tumor_subclusters["subclusters"].values() for idx in sub.values()]
+        cluster_by_groups = True
+    obs = [np.asarray(v) for v in obj.observation_grouped_cell_indices.values()]
+    refs = [np.asarray(v) for v in obj.reference_grouped_cell_indices.values()]
+    return (obs if cluster_by_groups else [np.asarray([c]) for c in np.concatenate(obs)]) + refs
+
+
+def _states_object(obj: Infercnv, S: np.ndarray) -> Infercnv:
+    out = copy.copy(obj)
+    st = S.astype(np.float64)
+    st[S == 255] = -1.0                          # the wire format's "unassigned" back to R's -1 (marshalling)
+    out.expr_data = np.asfortranarray(st)
+    return out
+
+
+def smooth_block_hmm(infercnv_obj: Infercnv, analysis_mode: str, cnv_mean_sd: dict, cnv_level_to_mean_sd_fit: dict,
+                     cluster_by_groups: bool = True, t: float = 1e-6, window_length: int = 101,
+                     max_centered_threshold: float = 3.0, apply_log: bool = True, use_bounds: bool = True):
+    """run() steps 4, 8-12, 14 and the i6 group-mode HMM of step 17 (predict_CNV_via_HMM_on_whole_tumor_samples or
+    ..._on_tumor_subclusters on the block's output) in one library call, for analysis_mode "samples" and "subclusters"
+    (random_trees subclusters, made before the block).  Returns (obj after step 14, states object); the hspike goes through
+    the plain block."""
+    obj = copy.copy(infercnv_obj)
+    cs, cl = obj.chr_ranges()
+    groups = _hmm_groups(obj, analysis_mode, cluster_by_groups)
+    Pi, delta, mean, _ = get_HMM(cnv_mean_sd, t)
+    sds = np.concatenate([_state_emission_sds(len(g), cnv_mean_sd, cnv_level_to_mean_sd_fit) for g in groups])
+    Y, S = api.smooth_hmm(obj.expr_data, cs, cl, _ref_groups(obj), Pi, delta, mean, sds, apply_log=apply_log,
+                          threshold=max_centered_threshold, window_length=window_length, use_bounds=use_bounds,
+                          groups=groups)
+    obj.expr_data = Y
+    hmm_obj = _states_object(obj, S)
+    if obj.hspike is not None:
+        obj.hspike = smooth_block(obj.hspike, window_length, max_centered_threshold, apply_log, use_bounds)
+    return obj, hmm_obj
+
+
 def smooth_block_i3_hmm(infercnv_obj: Infercnv, window_length: int = 101, max_centered_threshold: float = 3.0,
                         apply_log: bool = True, use_bounds: bool = True, i3_p_val: float = 0.05, t: float = 1e-6,
-                        median_filter_window: Optional[int] = None):
+                        median_filter_window: Optional[int] = None, analysis_mode: str = "cells",
+                        cluster_by_groups: bool = True):
     """The i3 counterpart of smooth_block: run() steps 4, 8-12, 14, .i3HMM_get_sd_trend_by_num_cells_fit on the block's
-    reference cells, the per-cell i3 HMM (i3HMM.R:180-225, use_KS = FALSE) and, with median_filter_window, the
+    reference cells, the i3 HMM (i3HMM.R:180-389, use_KS = FALSE) and, with median_filter_window, the
     apply_median_filtering of that window (noise_reduction.R:43-113, the lists of apply_median_filtering below) - one library
-    call.  Returns (obj after step 14, states object, median-filtered object or None, sd_trend); sd_trend's KS_delta is None
-    (it comes from R's RNG)."""
+    call.  analysis_mode "samples" / "subclusters" runs the group-mode HMM over the lists of smooth_block_hmm; the median
+    filter is then a second call on the block's output.  Returns (obj after step 14, states object, median-filtered object
+    or None, sd_trend); sd_trend's KS_delta is None (it comes from R's RNG)."""
     obj = copy.copy(infercnv_obj)
     cs, cl = obj.chr_ranges()
     lists = None
@@ -240,14 +288,19 @@ def smooth_block_i3_hmm(infercnv_obj: Infercnv, window_length: int = 101, max_ce
         subs = (obj.tumor_subclusters or {}).get("subclusters", {})
         lists = [np.asarray(idx) for tt in obj.observation_grouped_cell_indices for idx in subs.get(tt, {}).values()]
         lists += [np.asarray(idx) for idx in obj.reference_grouped_cell_indices.values()]
-    Y, S, F, model = api.smooth_i3_hmm(obj.expr_data, cs, cl, _ref_groups(obj), i3_p_val=i3_p_val, t=t, median_lists=lists,
-                                       median_window=median_filter_window or 7, apply_log=apply_log,
-                                       threshold=max_centered_threshold, window_length=window_length, use_bounds=use_bounds)
+    if analysis_mode != "cells":
+        Y, S, _, model = api.smooth_i3_hmm(obj.expr_data, cs, cl, _ref_groups(obj), i3_p_val=i3_p_val, t=t,
+                                           apply_log=apply_log, threshold=max_centered_threshold,
+                                           window_length=window_length, use_bounds=use_bounds,
+                                           groups=_hmm_groups(obj, analysis_mode, cluster_by_groups))
+        F = api.median_filter(Y, cs, cl, lists, median_filter_window) if lists is not None else None
+    else:
+        Y, S, F, model = api.smooth_i3_hmm(obj.expr_data, cs, cl, _ref_groups(obj), i3_p_val=i3_p_val, t=t,
+                                           median_lists=lists, median_window=median_filter_window or 7,
+                                           apply_log=apply_log, threshold=max_centered_threshold,
+                                           window_length=window_length, use_bounds=use_bounds)
     obj.expr_data = Y
-    hmm_obj = copy.copy(obj)
-    st = S.astype(np.float64)
-    st[S == 255] = -1.0
-    hmm_obj.expr_data = np.asfortranarray(st)
+    hmm_obj = _states_object(obj, S)
     med_obj = None
     if F is not None:
         med_obj = copy.copy(obj)
